@@ -6,7 +6,7 @@
 A "step" is one pass of the shading megakernel over one frame of a synthetic scene. The default workload is BASELINE config 3, the
 one the metric is quoted on: the Bistro-like city (2.8 M triangles) at 1920x1080, 8 quad lights, 64 spp, diffuse+specular MIS with the
 clamped optimal heuristic, shadow rays on. C2 (1 light, 4 spp, diffuse only) and C4 (the attic-like room at 3840x2160, 32 lights,
-256 spp: the configuration north_star shards over 8 GPUs) are selectable; results of those runs live under profiles/.
+256 spp: the configuration meant to be sharded over 8 GPUs) are selectable.
 
   value  whole-job Msamples/s (pixels*spp / time), inputs resident in HBM, CUDA events on the launching stream, L2 flushed between
          steps, max over ranks
@@ -14,6 +14,8 @@ clamped optimal heuristic, shadow rays on. C2 (1 light, 4 spp, diffuse only) and
   N > 1  every GPU shades the screen tiles (tx + ty / 8) % N == rank of the frame (strong scaling); the shading kernel stores finished pixels into
          the frames of all GPUs over NVLink (vkr_frame_exchange_t), two one-block kernels form the barrier: all of it inside the timed
          region. After the timed loop every rank's frame is hashed and compared with a single-GPU render of the same frame.
+  --dump-outputs DIR  writes the frame of the last timed step (what a caller of the shading pass receives) to DIR/frame.npy, float32
+         [height, width, 4]; frames above 64 MB are replaced by a fixed, seeded sample of 2^21 pixels (DIR/frame_sample.npy, [n, 4]).
 
 --impl reference times the reference's shader sources compiled for the CPU (oracle/_ref, all host threads) on a bounded sample of
 the same frame; the reference's Vulkan path itself cannot run on this box (no ICD, no glslangValidator).
@@ -114,7 +116,7 @@ def measured_peak():
 	if os.path.exists(path):
 		with open(path) as f:
 			return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-	return 6650.0, "fallback (B200_PROFILING.md)"
+	return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 def recorded_capture(workload):
@@ -181,7 +183,7 @@ def run_b200(args):
 	f0_lum = (gb[3, :, :, :3] * torch.tensor([0.2126, 0.7152, 0.0722], device=dev)).sum(-1)
 	ltc_layers = int(torch.unique(torch.round(f0_lum[valid].clamp(0, 1) * 50.0)).numel()) if bool(valid.any()) else 0
 	p = frame.create_pass(width, height, stripe_index=rank, stripe_count=world)
-	flush = torch.empty(512 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)  # > 126 MB L2
+	flush = torch.empty(512 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)  # > 50 MB L2
 
 	# --- N > 1: the frame exchange (peer stores from the kernel epilogue); the all_gather edition only if the GPUs cannot map each other's memory
 	exchange = None; gather = None; exchange_kind = "single GPU"
@@ -210,6 +212,13 @@ def run_b200(args):
 			assert rc == 0
 			if gather is not None:
 				gather.gather_frame(out)
+
+	def frame_bytes_of_this_rank():
+		if exchange is None:
+			return out.cpu().numpy().tobytes()
+		host = np.empty((height, width, 4), dtype=np.float32)
+		assert lib.vkr_frame_exchange_download(C.byref(exchange), C.byref(frame.device), host.ctypes.data) == 0
+		return host.tobytes()
 
 	def timed(step_fn, steps, warmup):
 		for _ in range(warmup):
@@ -247,6 +256,8 @@ def run_b200(args):
 	total_ms = timed(step_device, args.steps, 0)
 	launches = (int(p.kernel_launches) - launches_before) * world * (3 if exchange is not None else 1)   # every rank: the shading kernel (+ signal and wait of the exchange)
 	clocks = sampler.stop() if rank == 0 else None
+	if args.dump_outputs and rank == 0:
+		dump_frame(args.dump_outputs, frame_bytes_of_this_rank(), height, width)
 	# one more step to read the kernel's own duration on every rank
 	flush.zero_(); step_device(); lib.vkr_shading_pass_wait(C.byref(p), C.byref(frame.device))
 	if exchange is not None:
@@ -261,12 +272,6 @@ def run_b200(args):
 	value = samples / (ms_per_step * 1e-3) / 1e6
 
 	# --- the frame every rank holds now against a single-GPU render of the same frame (rank 0 renders it alone)
-	def frame_bytes_of_this_rank():
-		if exchange is None:
-			return out.cpu().numpy().tobytes()
-		host = np.empty((height, width, 4), dtype=np.float32)
-		assert lib.vkr_frame_exchange_download(C.byref(exchange), C.byref(frame.device), host.ctypes.data) == 0
-		return host.tobytes()
 	frame_check = None
 	if world > 1:
 		mine = hashlib.sha256(frame_bytes_of_this_rank()).hexdigest()
@@ -333,10 +338,10 @@ def run_b200(args):
 		capture = recorded_capture(args.workload) if world == 1 else {}
 		slowest_kernel_ms = max(kernel_ms_all)
 		achieved = bytes_alg / (slowest_kernel_ms * 1e-3) / 1e9 if world == 1 else bytes_alg / (ms_per_step * 1e-3) / 1e9
-		sm_clock_hz = (clocks.get("sm_mhz") or 1965.0) * 1e6 if clocks else 1965.0e6
+		sm_clock_hz = (clocks.get("sm_mhz") or 1980.0) * 1e6 if clocks else 1980.0e6
 		roofline = {"bound": "hbm", "achieved": round(achieved, 3), "peak": peak, "unit": "GB/s", "frac": round(achieved / peak, 6), "traffic": capture.get("dram_bytes_per_launch"),
 			"peak_source": peak_kind, "algorithmic_bytes": int(bytes_alg), "algorithmic_bytes_per_sample": round(bytes_alg / samples, 3),
-			"note": "the HBM line is the contract's; what bounds this kernel is instruction issue and the L1 data pipe (SURVEY 8d: ~0.5 GB of compulsory traffic against >1 G shadow rays), see `issue` and `trace`"}
+			"note": "compulsory HBM traffic over kernel time; the frame is far from bandwidth-bound (SURVEY 8d: ~0.5 GB of compulsory traffic against >1 G shadow rays), see `trace`"}
 		if trace is not None:
 			roofline["trace"] = trace
 		if capture:
@@ -354,7 +359,7 @@ def run_b200(args):
 			"metric": metric_text(w), "value": round(value, 3), "unit": "Msamples/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": round(ms_per_step, 4),
 			"higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
 			"config": {"workload": workload_text(args.workload, w, tri_count), "parallelism": exchange_kind,
-				"l2": "flushed between steps (512 MiB memset); inputs %d MB > 126 MB L2" % ((4 * width * height * 16 + 112 * tri_count) // 1000000),
+				"l2": "flushed between steps (512 MiB memset); inputs %d MB > 50 MB L2" % ((4 * width * height * 16 + 112 * tri_count) // 1000000),
 				"rays_per_sample_pair": 2 if w["strategy"] == DIFFUSE_SPECULAR_MIS else 1, "sample_pairs": width * height * lights * spp,
 				"tile_order": "tiles launched dearest first by the cost measured in the previous frame" if p.reorder_tiles else "row-major"},
 			"e2e": {"value": round(e2e_value, 3), "unit": "Msamples/s", "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h), "ms_per_step": round(e2e_ms, 4)},
@@ -382,6 +387,22 @@ def run_b200(args):
 		print(json.dumps(result), flush=True)
 	if not ok:
 		sys.exit(3)
+
+
+DUMP_LIMIT_BYTES = 64 * 1000 * 1000
+DUMP_SAMPLE_PIXELS = 1 << 21   # 32 MiB of float32 RGBA
+
+
+def dump_frame(directory, frame_bytes, height, width):
+	"""The frame of the last timed step as DIR/frame.npy (float32 RGBA, [height, width, 4]). A frame larger than 64 MB is replaced by a fixed
+	sample of its pixels (seeded, in raster order) as DIR/frame_sample.npy ([n, 4]), so that two builds can be compared output for output."""
+	os.makedirs(directory, exist_ok=True)
+	image = np.frombuffer(frame_bytes, dtype=np.float32).reshape(height, width, 4)
+	if image.nbytes <= DUMP_LIMIT_BYTES:
+		np.save(os.path.join(directory, "frame.npy"), image)
+		return
+	pixels = np.sort(np.random.default_rng(0).choice(height * width, DUMP_SAMPLE_PIXELS, replace=False))
+	np.save(os.path.join(directory, "frame_sample.npy"), image.reshape(-1, 4)[pixels])
 
 
 def host_threads():
@@ -514,7 +535,10 @@ def main():
 	ap.add_argument("--no-counters", action="store_true", help="skip the extra untimed launch of the counters edition of the kernel")
 	ap.add_argument("--cpu-port", action="store_true", help="time the C restatement (oracle/) on the CPU legs even if the compiled reference shader is available")
 	ap.add_argument("--cpu-band-stride", type=int, default=4, help="the CPU sample takes one 8-row band every this many tile rows")
+	ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the frame of the last timed step to DIR/frame.npy (float32; a fixed pixel sample above 64 MiB)")
 	args = ap.parse_args()
+	if args.dump_outputs and args.impl == "reference":
+		ap.error("--dump-outputs writes the frame of the CUDA path; --impl reference shades only bands of the frame on the host cores")
 	if args.warmup < 3:
 		log("[bench] note: the timing rules ask for at least 3 warm-up steps (got %d)" % args.warmup)
 	if args.impl == "reference":

@@ -1,4 +1,4 @@
-/* vkr_b200.h -- C-ABI of the B200-native shading pass (libvkr_b200.so).
+/* vkr_b200.h -- C-ABI of the H100-native (sm_90a) shading pass (libvkr_b200.so).
  *
  * Drop-in boundary for ONE path of MomentsInGraphics/vulkan_renderer: the per-pixel shading
  * pass (src/shaders/shading_pass.frag.glsl + polygon_sampling.glsl + the ray-query shadow test).
@@ -71,7 +71,7 @@ typedef enum vkr_noise_type_e { vkr_noise_type_white = 0, vkr_noise_type_blue = 
 /* ---- device (replaces create_vulkan_device, src/vulkan_basics.c:24; device_t, vulkan_basics.h:40-77) */
 typedef struct vkr_device_s {
 	int cuda_device;               /* ordinal handed to cudaSetDevice */
-	int sm_count;                  /* 148 on B200 */
+	int sm_count;                  /* 132 on H100 SXM */
 	int ray_tracing_supported;     /* always 1: the software BVH needs no RT cores (scene.c:485 gate) */
 	void* stream;                  /* cudaStream_t all asynchronous work is enqueued on */
 	int owns_stream;

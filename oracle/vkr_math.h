@@ -4,7 +4,7 @@
  * atan/sin/cos/acos/inversesqrt/normalize implementation-defined (GLSL.std.450,
  * un-pinned driver code, SURVEY 8c); this header pins ONE valid instance of
  * them built only from IEEE-754 correctly-rounded +,-,*,/,sqrt,fma so that the
- * same bits can be produced on x86 (gcc -ffp-contract=off -mfma) and on sm_100a
+ * same bits can be produced on x86 (gcc -ffp-contract=off -mfma) and on sm_90a
  * (nvcc -fmad=false, explicit fmaf). The CUDA path carries its OWN
  * implementation of the same definitions (vulkan_renderer_b200/csrc/
  * vkr_device_math.cuh); the two are compared bit-for-bit by tests/.

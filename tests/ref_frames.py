@@ -1,9 +1,22 @@
 """Frame set-up shared by tools/make_ref_golden.py and tests/test_ref_shader.py (host-only, no GPU)."""
 import ctypes as C
+import hashlib
+
+import numpy as np
 
 from vulkan_renderer_b200 import api
 
 WIDTH, HEIGHT = 64, 48
+
+
+def frame_sha256(frame):
+	"""What tests/golden/ref_shader.npz keeps of a frame of the reference shader (`<name>/rgba_sha256`): the SHA-256 of its float32 RGBA bytes."""
+	return hashlib.sha256(np.ascontiguousarray(frame, dtype=np.float32).tobytes()).digest()
+
+
+def assert_matches_fixture(golden, name, frame):
+	"""Bit for bit: the frame equals the reference shader's fixture `name`."""
+	assert frame_sha256(frame) == bytes(golden[name + "/rgba_sha256"]), "%s: the frame differs from the reference shader's" % name
 
 
 def dataset_for(cfg):

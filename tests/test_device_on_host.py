@@ -13,7 +13,7 @@ import numpy as np
 import pytest
 
 from tests import harness as H
-from tests.ref_frames import host_constants
+from tests.ref_frames import assert_matches_fixture, host_constants
 from oracle import binding as O
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -208,8 +208,7 @@ def test_error_display_light_shader_reproduces_the_reference_shader_fixtures(nam
 		C.c_uint32(cfg["error_display"]), C.c_int(cfg["show_lights"]), cb, P(gb), P(noise), C.c_uint32(noise.shape[2]), C.c_uint32(noise.shape[1]), C.c_uint32(noise.shape[0]),
 		P(ltc0), P(ltc1), C.c_uint32(ltc0.shape[1]), C.c_uint32(ltc0.shape[0]), P(out))
 	assert rc == 0
-	ref = g[name + "/rgba"]
-	assert np.array_equal(out.view(np.uint32), ref.view(np.uint32)), H.compare_radiance(out, ref)
+	assert_matches_fixture(g, name, out)
 
 
 def _base_fixture_names():
@@ -246,8 +245,7 @@ def test_shade_light_without_rays_matches_oracle_and_fixtures(name):
 	ref, _ = oi.shade(oracle_cfg(no_rays), constants, gb)
 	assert np.array_equal(out.view(np.uint32), ref.view(np.uint32)), H.compare_radiance(out, ref)
 	if cfg["trace"] == 0:
-		fixture = g[name + "/rgba"]
-		assert np.array_equal(out.view(np.uint32), fixture.view(np.uint32)), H.compare_radiance(out, fixture)
+		assert_matches_fixture(g, name, out)
 
 
 def _related_work_fixture_names():
@@ -282,8 +280,7 @@ def test_related_work_light_shader_without_rays_matches_oracle_and_fixtures(name
 	ref, _ = oi.shade(oracle_cfg(dict(cfg, trace=0)), constants, gb)
 	assert np.array_equal(out.view(np.uint32), ref.view(np.uint32)), H.compare_radiance(out, ref)
 	if cfg["trace"] == 0:
-		fixture = g[name + "/rgba"]
-		assert np.array_equal(out.view(np.uint32), fixture.view(np.uint32)), H.compare_radiance(out, fixture)
+		assert_matches_fixture(g, name, out)
 
 
 def _textured_light_fixture_names():
@@ -322,8 +319,7 @@ def test_textured_lights_without_rays_match_oracle_and_fixtures(name):
 	ref, _ = oi.shade(oracle_cfg(dict(cfg, trace=0)), constants, gb)
 	assert np.array_equal(out.view(np.uint32), ref.view(np.uint32)), H.compare_radiance(out, ref)
 	if cfg["trace"] == 0:
-		fixture = g[name + "/rgba"]
-		assert np.array_equal(out.view(np.uint32), fixture.view(np.uint32)), H.compare_radiance(out, fixture)
+		assert_matches_fixture(g, name, out)
 	# the textures matter: the same frame with white textures differs
 	white, _ = H.oracle.shade(oracle_cfg(dict(cfg, trace=0)), constants, gb, oi.noise, oi.ltc0, oi.ltc1, np.zeros((0, 9), dtype=np.float32),
 		light_textures=(np.array([[1, 1, 1]] * len(dims), dtype=np.uint32), np.arange(len(dims), dtype=np.uint64) * 4, np.ones(4 * len(dims), dtype=np.float32)))

@@ -1,6 +1,6 @@
 """Randomised differential tests (tools/fuzz_parity.py): random cameras, lights and settings on random shader configurations.
-(1) the device code compiled for the CPU against the oracle -- runs everywhere; (2) the reference shader compiled as C++ against the oracle -- where
-oracle/_ref is built. Bit for bit. The tool itself runs hundreds of frames (python tools/fuzz_parity.py --frames 500); these are short samples of it."""
+(1) the device code compiled for the CPU against the oracle; (2) the reference shader compiled as C++ (its frames frozen as digests) against the
+oracle. Bit for bit. The tool itself runs hundreds of frames (python tools/fuzz_parity.py --frames 500); these are short samples of it."""
 import os
 import sys
 
@@ -9,8 +9,9 @@ import pytest
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 
+import numpy as np  # noqa: E402
+
 import fuzz_parity  # noqa: E402
-from oracle import ref_binding as R  # noqa: E402
 
 
 def test_device_code_matches_the_oracle_on_random_frames():
@@ -27,8 +28,12 @@ def test_device_code_matches_the_oracle_on_any_legal_configuration():
 	assert not any(mismatches.values())
 
 
-@pytest.mark.skipif(not R.available(), reason="oracle/_ref/libref_shader.so not built (needs /root/reference)")
+REFERENCE_RUN = dict(frames=16, seed=202)
+
+
 def test_oracle_matches_the_reference_shader_on_random_frames():
-	mismatches, compared, lit = fuzz_parity.run(frames=16, seed=202, with_reference=True, verbose=False)
+	"""The reference shader's frames of this run are frozen as SHA-256 digests in tests/golden/ref_live.npz (tools/make_ref_live_golden.py)."""
+	frozen = [bytes(d).hex() for d in np.load(os.path.join(ROOT, "tests", "golden", "ref_live.npz"))["fuzz/reference_sha256"]]
+	mismatches, compared, lit = fuzz_parity.run(with_reference=False, verbose=False, reference_digests=frozen, **REFERENCE_RUN)
 	assert compared["reference vs oracle"] == 16 and lit >= 12
 	assert not any(mismatches.values())

@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 from tests import harness as H
+from tests.ref_frames import assert_matches_fixture
 from vulkan_renderer_b200 import api
 
 pytestmark = pytest.mark.gpu
@@ -107,7 +108,4 @@ def test_cuda_path_reproduces_reference_shader_fixture(name):
 		out = frame.shade_host(WIDTH, HEIGHT, gb)
 	finally:
 		frame.close()
-	ref = g[name + "/rgba"]
-	cmp = H.compare_radiance(out, ref, rel=REL_TOL)
-	assert cmp["bad_pixels"] == 0 and cmp["nan_mismatch"] == 0, cmp
-	assert cmp["bit_exact"], cmp
+	assert_matches_fixture(g, name, out)

@@ -1,13 +1,14 @@
 """Textured polygonal lights on the GPU (get_polygon_radiance, shading_pass.frag.glsl:151-185: area texture, portal onto a light probe, IES profile):
 textured_light_kernel (csrc/vkr_textured_light_kernel.cu) against frames of the REFERENCE's own shader sources fed with the same textures (fixtures
 "_y1", tests/test_ref_shader.py) -- bit-identical -- and against the oracle on a larger frame. The per-pixel code underneath is also run on the CPU
-(tests/test_device_on_host.py). Written after this round's GPU budget was spent: it has not run on a B200 yet, hence its place late in the order."""
+(tests/test_device_on_host.py). Placed late in the order."""
 import os
 
 import numpy as np
 import pytest
 
 from tests import harness as H
+from tests.ref_frames import assert_matches_fixture
 from vulkan_renderer_b200 import api
 
 pytestmark = pytest.mark.gpu
@@ -39,8 +40,7 @@ def test_textured_lights_reproduce_reference_shader_fixture(name):
 		out = frame.shade_host(WIDTH, HEIGHT, gb)
 	finally:
 		frame.close()
-	ref = g[name + "/rgba"]
-	assert np.array_equal(out.view(np.uint32), ref.view(np.uint32)), H.compare_radiance(out, ref)
+	assert_matches_fixture(g, name, out)
 
 
 @pytest.mark.parametrize("technique", [api.TECHNIQUE_PSA, api.TECHNIQUE_PSA_BIASED])

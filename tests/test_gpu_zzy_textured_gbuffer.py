@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 from tests import harness as H
+from tests.ref_frames import assert_matches_fixture
 from vulkan_renderer_b200 import api
 
 pytestmark = pytest.mark.gpu
@@ -39,8 +40,7 @@ def test_textured_frame_reproduces_reference_shader_fixture(name):
 		out = frame.shade_host(WIDTH, HEIGHT, gb)
 	finally:
 		frame.close()
-	ref = g[name + "/rgba"]
-	assert np.array_equal(out.view(np.uint32), ref.view(np.uint32)), H.compare_radiance(out, ref)
+	assert_matches_fixture(g, name, out)
 
 
 def test_textured_gbuffer_matches_the_oracle_and_differs_from_constant_materials():

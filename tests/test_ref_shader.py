@@ -1,6 +1,6 @@
 """Pins the CPU oracle against the REFERENCE's own shader sources.
 
-tests/golden/ref_shader.npz holds frames shaded by src/shaders/shading_pass.frag.glsl (+ includes) compiled as C++
+tests/golden/ref_shader.npz holds (SHA-256 digests of) frames shaded by src/shaders/shading_pass.frag.glsl (+ includes) compiled as C++
 (oracle/build_ref.py, oracle/glsl_compat/). The oracle must reproduce them bit for bit, for every sampling strategy
 and MIS heuristic of the projected-solid-angle technique and for the related-work techniques ("_q<technique>": Turk, Urena, Arvo, Hart; SURVEY 8 f4). Where oracle/_ref/libref_shader.so is present (build
 container, or shipped prebuilt) the reference shader is also run live and checked against the fixtures.
@@ -14,10 +14,11 @@ import numpy as np
 import pytest
 
 from tests import harness as H
-from tests.ref_frames import WIDTH, HEIGHT, dataset_for, host_constants, oracle_cfg
+from tests.ref_frames import WIDTH, HEIGHT, assert_matches_fixture, dataset_for, frame_sha256, host_constants, oracle_cfg
 from oracle import ref_binding as R
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_shader.npz")
+LIVE_GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_live.npz")
 
 
 def _golden():
@@ -47,9 +48,8 @@ def test_oracle_reproduces_reference_shader_bit_for_bit(name):
 	assert np.array_equal(vis, g[name + "/visibility"])
 	gb = oi.gbuffer(WIDTH, HEIGHT, constants, vis)
 	out, _ = oi.shade(oracle_cfg(cfg), constants, gb)
-	ref = g[name + "/rgba"]
-	assert np.array_equal(out.view(np.uint32), ref.view(np.uint32)), H.compare_radiance(out, ref)
-	assert float(ref[..., :3].max()) > 0.0
+	assert_matches_fixture(g, name, out)
+	assert float(out[..., :3].max()) > 0.0
 
 
 @pytest.mark.skipif(not R.available(), reason="oracle/_ref/libref_shader.so not built (needs /root/reference)")
@@ -64,30 +64,32 @@ def test_live_reference_shader_matches_fixture():
 		info = H.dataset(dataset_for(cfg)); oi = H.OracleInputs(info)
 		constants = bytes(g[name + "/constants"])
 		ref = R.shade(cfg["entry"], WIDTH, HEIGHT, cfg, constants, g[name + "/visibility"], oi.vks, oi.material_params, oi.noise, oi.ltc0, oi.ltc1, oi.shadow_tris, textures=oi.textures, light_textures=oi.light_textures)
-		assert np.array_equal(ref.view(np.uint32), g[name + "/rgba"].view(np.uint32)), name
+		assert frame_sha256(ref) == bytes(g[name + "/rgba_sha256"]), name
 		checked += 1
 	assert checked > 0
 
 
-@pytest.mark.skipif(not R.available(), reason="oracle/_ref/libref_shader.so not built (needs /root/reference)")
-@pytest.mark.parametrize("width,height", [(40, 30), (97, 41)])
+OTHER_RESOLUTIONS = [(40, 30), (97, 41)]
+OTHER_RESOLUTION_PICKS = ["s0_h0_b0_L3_V4_S3_t1_l1_M8", "s1_h1_b0_L3_V4_S3_t1_l1_M8", "s2_h0_b0_L3_V4_S3_t1_l1_M8", "s3_h3_b0_L3_V4_S3_t1_l1_M8", "s4_h0_b0_L3_V4_S3_t1_l1_M8",
+	"s3_h4_b0_L3_V4_S3_t1_l1_M8", "s3_h3_b1_L3_V4_S3_t1_l1_M8", "s3_h3_b0_L3_V7m5_S3_t1_l1_M8", "s3_h3_b0_L32_V4_S2_t1_l1_M8",
+	"s0_h0_b0_L3_V4_S3_t1_l1_M8_q3", "s0_h0_b0_L3_V4_S3_t1_l1_M8_q9", "s1_h0_b0_L3_V4_S3_t1_l1_M8_q10", "s0_h0_b0_L3_V7m5_S3_t1_l1_M8_q7",
+	"s3_h3_b0_L3_V4_S3_t1_l1_M8_e4", "s3_h3_b0_L3_V4_S3_t1_l1_M8_x1"]
+
+
+@pytest.mark.parametrize("width,height", OTHER_RESOLUTIONS)
 def test_oracle_follows_the_live_reference_shader_at_other_resolutions(width, height):
 	"""The fixtures are 64x48; other resolutions move every pixel ray, sample and noise fetch. A spread of configurations (every strategy,
-	related-work techniques, error display, textures) is shaded by the reference shader and by the oracle: bit-identical again."""
-	picks = ["s0_h0_b0_L3_V4_S3_t1_l1_M8", "s1_h1_b0_L3_V4_S3_t1_l1_M8", "s2_h0_b0_L3_V4_S3_t1_l1_M8", "s3_h3_b0_L3_V4_S3_t1_l1_M8", "s4_h0_b0_L3_V4_S3_t1_l1_M8",
-		"s3_h4_b0_L3_V4_S3_t1_l1_M8", "s3_h3_b1_L3_V4_S3_t1_l1_M8", "s3_h3_b0_L3_V7m5_S3_t1_l1_M8", "s3_h3_b0_L32_V4_S2_t1_l1_M8",
-		"s0_h0_b0_L3_V4_S3_t1_l1_M8_q3", "s0_h0_b0_L3_V4_S3_t1_l1_M8_q9", "s1_h0_b0_L3_V4_S3_t1_l1_M8_q10", "s0_h0_b0_L3_V7m5_S3_t1_l1_M8_q7",
-		"s3_h3_b0_L3_V4_S3_t1_l1_M8_e4", "s3_h3_b0_L3_V4_S3_t1_l1_M8_x1"]
-	live = {c["name"]: c for c in R.configs()}
-	for name in picks:
-		cfg = live[name]
+	related-work techniques, error display, textures) shaded by the reference shader (frozen as SHA-256 digests of its float32 frames in
+	tests/golden/ref_live.npz by tools/make_ref_live_golden.py) and by the oracle: bit-identical again."""
+	frozen = np.load(LIVE_GOLDEN)
+	for name in OTHER_RESOLUTION_PICKS:
+		cfg = _config_from_name(name)
 		info = H.dataset(dataset_for(cfg)); oi = H.OracleInputs(info)
 		constants = host_constants(info, width, height, cfg["lights"])
 		vis = oi.visibility(width, height, constants)
-		ref = R.shade(cfg["entry"], width, height, cfg, constants, vis, oi.vks, oi.material_params, oi.noise, oi.ltc0, oi.ltc1, oi.shadow_tris, textures=oi.textures, light_textures=oi.light_textures)
 		gb = oi.gbuffer(width, height, constants, vis)
 		out, _ = oi.shade(oracle_cfg(cfg, width, height), constants, gb)
-		assert np.array_equal(out.view(np.uint32), ref.view(np.uint32)), (name, H.compare_radiance(out, ref))
+		assert frame_sha256(out) == frozen["shader/%dx%d/%s" % (width, height, name)].tobytes(), name
 
 
 def test_every_light_texturing_technique_shapes_the_textured_fixture():
@@ -98,7 +100,8 @@ def test_every_light_texturing_technique_shapes_the_textured_fixture():
 	assert [l["texturing_technique"] for l in info["lights"][:3]] == [1, 2, 3]
 	constants = bytes(g[name + "/constants"])
 	gb = oi.gbuffer(WIDTH, HEIGHT, constants, g[name + "/visibility"])
-	ref = g[name + "/rgba"]
+	ref, _ = oi.shade(oracle_cfg(cfg), constants, gb)
+	assert_matches_fixture(g, name, ref)
 	dims, offsets, data = oi.light_textures
 	for i in range(3):
 		d = dims.copy(); o = offsets.copy(); white = np.concatenate([data, np.ones(4, dtype=np.float32)])

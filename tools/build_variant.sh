@@ -7,7 +7,7 @@ set -e
 cd "$(dirname "$0")/.."
 name=$1; flags=$2
 out=vulkan_renderer_b200/variants; mkdir -p $out
-common="-gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -fmad=false -prec-div=true -prec-sqrt=true -ftz=false -ccbin /usr/bin/g++ -Xcompiler -fPIC -I include"
+common="-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -fmad=false -prec-div=true -prec-sqrt=true -ftz=false -ccbin /usr/bin/g++ -Xcompiler -fPIC -I include"
 nvcc $common -DVKR_MAXP_TU=5 $flags -c vulkan_renderer_b200/csrc/vkr_shading_kernel.cu -o $out/$name.o
 nvcc $common -DVKR_MAXP_TU=5 -DVKR_TRACE_STATS=1 $flags -c vulkan_renderer_b200/csrc/vkr_shading_kernel.cu -o $out/${name}_stats.o
 [ -f $out/stubs.o ] || nvcc $common -c tools/variant_stubs.cu -o $out/stubs.o

@@ -9,6 +9,7 @@ scaled lights (also behind surfaces, grazing, partly below horizons), random exp
   (2) the DEVICE code compiled for the CPU (tests/device_on_host.cpp, rays off)  vs  the oracle -- the arithmetic the GPU kernels run.
 All comparisons are bit for bit. Prints one line per mismatch and a summary; exit code 1 if anything differs."""
 import argparse
+import hashlib
 import re
 import ctypes as C
 import os
@@ -183,8 +184,10 @@ def random_config(rng):
 	return cfg
 
 
-def run(frames, seed, width=48, height=32, max_samples=8, with_reference=True, verbose=True, only=None, wild=False, any_config=False):
-	"""Returns (mismatches, compared): dicts with the keys "reference vs oracle" and "device code vs oracle"."""
+def run(frames, seed, width=48, height=32, max_samples=8, with_reference=True, verbose=True, only=None, wild=False, any_config=False, record_digests=None, reference_digests=None):
+	"""Returns (mismatches, compared): dicts with the keys "reference vs oracle" and "device code vs oracle".
+	record_digests: a list that receives the SHA-256 (hex) of every frame of the reference shader. reference_digests: such a list from an earlier
+	run with the same arguments (tests/golden/ref_live.npz); the oracle's frames are held against it where the reference shader is not built."""
 	import __graft_entry__
 	dev = C.CDLL(__graft_entry__.build_device_on_host())
 	rng = np.random.default_rng(seed)
@@ -220,10 +223,17 @@ def run(frames, seed, width=48, height=32, max_samples=8, with_reference=True, v
 		lit += int((out[..., :3].sum(-1) > 0).any()); pink += int(((out[..., 1] == 0) & (out[..., 0] > 0) & (out[..., 2] > 0)).any())
 		if with_reference:
 			ref = R.shade(cfg["entry"], width, height, cfg, constants, vis, oi.vks, oi.material_params, oi.noise, oi.ltc0, oi.ltc1, oi.shadow_tris, textures=oi.textures, light_textures=oi.light_textures)
+			if record_digests is not None:
+				record_digests.append(hashlib.sha256(ref.tobytes()).hexdigest())
 			compared["reference vs oracle"] += 1
 			if not np.array_equal(out.view(np.uint32), ref.view(np.uint32)):
 				mismatches["reference vs oracle"] += 1
 				print("MISMATCH reference vs oracle: frame %d seed %d %s %dx%d %s" % (f, seed, cfg["name"], width, height, H.compare_radiance(out, ref)), flush=True)
+		elif reference_digests is not None:
+			compared["reference vs oracle"] += 1
+			if hashlib.sha256(np.ascontiguousarray(out, dtype=np.float32).tobytes()).hexdigest() != reference_digests[f]:
+				mismatches["reference vs oracle"] += 1
+				print("MISMATCH reference (frozen) vs oracle: frame %d seed %d %s %dx%d" % (f, seed, cfg["name"], width, height), flush=True)
 		host = device_on_host_frame(dev, cfg, oi, constants, gb, width, height)
 		if host is not None:
 			no_rays, _ = oi.shade(oracle_cfg(dict(cfg, trace=0), width, height), constants, gb)

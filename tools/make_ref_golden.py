@@ -4,7 +4,7 @@
   python tools/make_ref_golden.py        (needs /root/reference; run in the build container)
 
 For every configuration in oracle/_ref/configs.json a 64x48 frame of a seeded synthetic scene is shaded by the
-reference shader; inputs are identified by sha256 of the scene file and the constant block is stored, so a drift
+reference shader and kept as the SHA-256 of its float32 RGBA bytes; inputs are identified by sha256 of the scene file and the constant block is stored, so a drift
 of the synthetic-data generator is detected instead of silently changing the fixture's meaning.
 Output: tests/golden/ref_shader.npz (committed).
 """
@@ -18,7 +18,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from tests import harness as H  # noqa: E402
-from tests.ref_frames import WIDTH, HEIGHT, dataset_for, host_constants  # noqa: E402
+from tests.ref_frames import WIDTH, HEIGHT, dataset_for, frame_sha256, host_constants  # noqa: E402
 from oracle import ref_binding as R  # noqa: E402
 
 
@@ -35,7 +35,7 @@ def main():
 		vis = oi.visibility(WIDTH, HEIGHT, constants)
 		ref = R.shade(cfg["entry"], WIDTH, HEIGHT, cfg, constants, vis, oi.vks, oi.material_params, oi.noise, oi.ltc0, oi.ltc1, oi.shadow_tris, textures=oi.textures, light_textures=oi.light_textures)
 		key = cfg["name"]
-		out[key + "/rgba"] = ref
+		out[key + "/rgba_sha256"] = np.frombuffer(frame_sha256(ref), dtype=np.uint8)   # the frame itself: bit-identical or not, in 32 bytes
 		out[key + "/visibility"] = vis
 		out[key + "/constants"] = np.frombuffer(constants, dtype=np.uint8)
 		out[key + "/vks_sha256"] = np.frombuffer(hashlib.sha256(open(info["vks"], "rb").read()).digest(), dtype=np.uint8)

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Runs the reference's experiment list (src/experiment_list.c) on the B200 path and writes the timing matrix as JSON.
+"""Runs the reference's experiment list (src/experiment_list.c) on the CUDA path and writes the timing matrix as JSON.
 
   python tools/run_experiments.py --out gpurun_out/experiments [--select timings_central_4] [--width 1920 --height 1080] [--frames 12] [--no-screenshots]
 

@@ -26,22 +26,23 @@ def main():
 	ops = collections.Counter(re.sub(r"^@!?U?P\d\s+", "", l.split("*/", 1)[1].strip()).split()[0].rstrip(";") for l in lines)
 	def family(prefixes): return sum(v for k, v in ops.items() if k.split(".")[0] in prefixes)
 	git = subprocess.run(["git", "-C", ROOT, "rev-parse", "--short", "HEAD"], stdout=subprocess.PIPE, text=True).stdout.strip()
-	out = ["# SASS of `shading_kernel<3,5,0,0,1>` (sm_100a), commit %s" % git, "",
+	out = ["# SASS of `shading_kernel<3,5,0,0,1>` (sm_90a), commit %s" % git, "",
 		"`cuobjdump -sass -fun %s vulkan_renderer_b200/build/vkr_shading_kernel_maxp5.cu.o`, excerpts." % KERNEL, "",
 		"* resource usage: `%s`" % (usage[0] if usage else "?"),
-		"* %d instructions; FFMA / FMUL / FADD %d, FMNMX / FMNMX3 %d, MUFU %d, LDG %d (of them 256-bit: %d), LDS / STS %d, LDL / STL (spills) %d, VOTE / SHFL %d" % (
-			len(lines), family({"FFMA", "FMUL", "FADD"}), family({"FMNMX", "FMNMX3"}), family({"MUFU"}), family({"LDG"}), sum(v for k, v in ops.items() if k.startswith("LDG") and ".256" in k),
+		"* %d instructions; FFMA / FMUL / FADD %d, FMNMX %d, MUFU %d, LDG %d (of them 128-bit: %d), LDS / STS %d, LDL / STL (spills) %d, VOTE / SHFL %d" % (
+			len(lines), family({"FFMA", "FMUL", "FADD"}), family({"FMNMX"}), family({"MUFU"}), family({"LDG"}), sum(v for k, v in ops.items() if k.startswith("LDG") and ".128" in k),
 			family({"LDS", "STS"}), family({"LDL", "STL"}), family({"VOTE", "VOTEU", "SHFL"})),
-		"* no tensor-core, TMEM or tensor-map instructions (HMMA / UTCMMA / UTMALDG count: %d): the path has no contraction" % family({"HMMA", "UTCHMMA", "UTCMMA", "UTMALDG", "UTCQMMA"}), ""]
+		"* no tensor-core or tensor-map instructions (HMMA / HGMMA / UTMALDG count: %d): the path has no contraction" % family({"HMMA", "HGMMA", "UTMALDG"}), ""]
 	def excerpt(title, pattern, before, after, limit=1):
 		hits = [i for i, l in enumerate(lines) if re.search(pattern, l)][:limit]
 		for i in hits:
 			out.extend(["## %s" % title, "", "```"] + lines[max(0, i - before):i + after + 1] + ["```", ""])
 	excerpt("Constant block: one bulk asynchronous copy into shared memory, completion on an mbarrier", r"UBLKCP", 6, 8)
 	excerpt("Role split: trace warps give registers to the shading warps", r"USETMAXREG", 2, 3, limit=2)
-	excerpt("Trace warps: the node loop (one node pair = two 256-bit loads; slab test as FFMA + FMNMX3; shared-memory stack)", r"LDG\.E\.ENL2\.256", 4, 62)
+	excerpt("Trace warps: the node loop (one node pair = four 128-bit loads; slab test as FFMA + FMNMX; shared-memory stack)", r"LDG\.E\.128\.CONSTANT", 4, 62)
 	excerpt("Trace warps: ticket draw (one shared-memory atomic per warp refill)", r"ATOMS\.ADD", 8, 6)
 	path = os.path.join(ROOT, "profiles", "%s_sass_excerpt.md" % tag)
+	os.makedirs(os.path.dirname(path), exist_ok=True)
 	with open(path, "w") as f:
 		f.write("\n".join(out) + "\n")
 	print("wrote", path, "(%d instructions)" % len(lines))

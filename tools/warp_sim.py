@@ -6,7 +6,7 @@
 Builds the benchmark scene (C3), takes 48 random 8x4 pixel patches of its G-buffer and generates the shadow rays of 12 sample pairs per light in the order the
 shading warps submit them; 32 emulated lanes then run the per-lane state machine of vkr_ray_stream.cuh (tickets, occluder cache, slab set-up, node loop with
 the postponed leaf, leaf tests, anchored starts) with phases costed in warp instructions taken from the kernel's SASS. The baseline reproduces what ncu
-measured on the B200 in round 1 (24.2 vs 23.7 lanes per node step, 13.2 vs 13.4 lanes per triangle test, 4444 vs ~4270 warp instructions per 32 rays), which
+measured on the GPU in an earlier round (24.2 vs 23.7 lanes per node step, 13.2 vs 13.4 lanes per triangle test, 4444 vs ~4270 warp instructions per 32 rays), which
 is what makes its verdicts on variants (refill thresholds, one leaf per round, anchored rays) worth having before GPU time is spent on them."""
 import ctypes as C, os, subprocess, sys, time
 import numpy as np

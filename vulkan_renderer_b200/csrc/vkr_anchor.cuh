@@ -134,7 +134,7 @@ template <class Push>
 VKR_DEV int visit_pair(const float4* __restrict__ nodes, int pair, int skip, const ray_slabs& r, float tmin, float tmax, Push&& push) {
 	const float4* nd = nodes + 4 * (size_t) pair;
 	float4 q0, q1, q2, q3;
-	ldg_256(nd, q0, q1); ldg_256(nd + 2, q2, q3);
+	ldg_32_bytes(nd, q0, q1); ldg_32_bytes(nd + 2, q2, q3);
 	const int ref0 = __float_as_int(q3.x), ref1 = __float_as_int(q3.y);
 	float tn0, tn1;
 	const bool h0 = ray_box(q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, r, tmin, tmax, &tn0) && skip != 0;

@@ -475,7 +475,7 @@ extern "C" int vkr_probe_rsqrt_exhaustive(const vkr_device_t* device, uint64_t* 
 	VKR_CUDA_OK(cudaMalloc(&d_count, sizeof(unsigned long long)), "Failed to allocate the probe's counter");
 	if (cudaMalloc(&d_first, sizeof(unsigned int)) != cudaSuccess) { cudaFree(d_count); printf("Failed to allocate the probe's result.\n"); return 1; }
 	cudaMemsetAsync(d_count, 0, sizeof(unsigned long long), stream); cudaMemsetAsync(d_first, 0xff, sizeof(unsigned int), stream);
-	vkr::rsqrt_probe_kernel<<<148 * 8, 256, 0, stream>>>(d_count, d_first);
+	vkr::rsqrt_probe_kernel<<<(device->sm_count > 0 ? device->sm_count : 132) * 8, 256, 0, stream>>>(d_count, d_first);
 	cudaError_t err = cudaGetLastError();
 	unsigned long long count = 0; unsigned int first = 0;
 	cudaMemcpyAsync(&count, d_count, sizeof(count), cudaMemcpyDeviceToHost, stream); cudaMemcpyAsync(&first, d_first, sizeof(first), cudaMemcpyDeviceToHost, stream);

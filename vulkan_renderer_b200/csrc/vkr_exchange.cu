@@ -1,6 +1,6 @@
 // vkr_exchange.cu -- one frame on several GPUs of a box: the frame exchange (include/vkr_b200.h, vkr_frame_exchange_t).
 //
-// The reference renders on one GPU (render_frame, src/main.c:2197-2270); SURVEY 8e adds the split over the GPUs of a B200 box. Every GPU shades
+// The reference renders on one GPU (render_frame, src/main.c:2197-2270); SURVEY 8e adds the split over the GPUs of an HGX box. Every GPU shades
 // its share of the screen tiles and the shading kernel's epilogue stores each finished pixel into the frame of EVERY GPU -- its own and, through
 // peer mappings over NVLink / NVSwitch, the others' (vkr_shading_tile.cuh, out_peers). What is left to do per frame is a barrier, made of two
 // one-block kernels on the launching stream:

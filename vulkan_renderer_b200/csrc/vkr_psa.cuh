@@ -1,4 +1,4 @@
-// vkr_psa.cuh -- projected-solid-angle sampling of convex polygons for sm_100a.
+// vkr_psa.cuh -- projected-solid-angle sampling of convex polygons for sm_90a.
 //
 // Implements the numerical recipe of Peters, "BRDF Importance Sampling for Polygonal Lights"
 // (SIGGRAPH 2021) as the reference renderer evaluates it

@@ -51,9 +51,9 @@ constexpr int kNodeLoopMinLanes = VKR_NODE_LOOP_MIN_LANES;
 #ifndef VKR_REFILL_MIN_LANES
 #define VKR_REFILL_MIN_LANES 1
 #endif
-// 1 (default since the last GPU visit of round 2: -4.3 % frame time): the decisions at the end of a node visit -- which child is entered, what is pushed, when the
-// stack is popped, the leaf that is put aside -- are written as predicated instructions (inline PTX) instead of an if / else chain: no divergent branch with
-// its BSSY / BRA / BSYNC inside the visit, 54 instead of 59 instructions. 0 keeps the C++ form (the anchored and 4-wide editions need it).
+// 1 (default): the decisions at the end of a node visit -- which child is entered, what is pushed, when the stack is popped, the leaf that is put aside --
+// are written as predicated instructions (inline PTX) instead of an if / else chain: no divergent branch with its BSSY / BRA / BSYNC inside the visit.
+// 0 keeps the C++ form (the anchored and 4-wide editions need it).
 #ifndef VKR_LEAN_NODE_STEP
 #define VKR_LEAN_NODE_STEP (!VKR_ANCHORED && VKR_BVH_WIDTH == 2)
 #endif
@@ -71,8 +71,8 @@ constexpr int kNodeLoopMinLanes = VKR_NODE_LOOP_MIN_LANES;
 #define VKR_TRACE_RELOAD_RAY 0
 #endif
 // The four shading warps of a CTA can walk their sample loop in loose lock step (a named barrier per iteration: 1 = per sample pair, 2 = per technique),
-// so that they fetch the loop's 32 KB of instructions together instead of four times: the SM's instruction cache is 32 KB and ncu shows the next level
-// (the GPC's) at 90 % of its request rate. Only tiles in which all four warps have pixels to shade use it (the barrier needs all of them).
+// so that they fetch the loop's 32 KB of instructions together instead of four times. Only tiles in which all four warps have pixels to shade use it
+// (the barrier needs all of them).
 #ifndef VKR_SHADING_LOCKSTEP
 #define VKR_SHADING_LOCKSTEP 0
 #endif
@@ -84,15 +84,14 @@ VKR_DEV void shading_lockstep_barrier() {
 	asm volatile("bar.sync 1, 128;" ::: "memory");
 #endif
 }
-// 1: the trace warps walk the quantised node pairs (32 bytes, vkr_trace.cuh) instead of the float pairs. Measured on the B200 (profiles/r02_variants.md): half
-// the bytes per visit, bit-identical frames, 2.7 % SLOWER (4 more instructions per visit, 6 % more triangle tests behind the fatter boxes) -- the kernel is not
-// bound by the L1 data pipe after all. Kept as a compile-time edition; not with anchored rays or the 4-wide variant.
+// 1: the trace warps walk the quantised node pairs (32 bytes, vkr_trace.cuh) instead of the float pairs: half the bytes per visit, bit-identical frames,
+// but more instructions per visit and more triangle tests behind the fatter boxes. Kept as a compile-time edition; not with anchored rays or the 4-wide variant.
 #ifndef VKR_QUANTISED_NODES
 #define VKR_QUANTISED_NODES 0
 #endif
-// 1 (default: another -1.4 %): the trace warps walk the interleaved node pairs (vkr_trace.cuh: the two children's numbers side by side, so that the slab
-// arithmetic of both children is 9 packed FMAs instead of 18 scalar ones) instead of the plain float pairs. Measured on the B200 (profiles/r02_variants.md):
-// 371.6 ms (C++ step, float pairs) -> 355.7 (predicated step) -> 350.6 (+ packed FMAs); FFMA2 evidently costs more than one issue slot, hence the small second step.
+// 1 (default): the trace warps walk the interleaved node pairs (vkr_trace.cuh: the two children's numbers side by side) instead of the plain float pairs.
+// Bit-identical frames either way. On an H100 (SXM, 700 W) the C3 frame takes 396.1 - 396.4 ms with them and 400.9 - 404.2 ms with the plain pairs
+// (tools/build_variant.sh + tools/quick_time.py, steady-state frames of two alternating runs each), worth the second copy of the pairs made at scene load.
 #ifndef VKR_INTERLEAVED_NODES
 #define VKR_INTERLEAVED_NODES (!VKR_ANCHORED && !VKR_QUANTISED_NODES && VKR_BVH_WIDTH == 2)
 #endif
@@ -490,15 +489,15 @@ VKR_DEV void trace_stream(const uint32_t base, const float4* __restrict__ nodes,
 			if ((__activemask() & lt_mask) == 0u) VKR_STAT(st_node_iters);
 #if VKR_QUANTISED_NODES
 			float4 q0, q1;   // one 32-byte pair: six words of 16-bit box coordinates, two references
-			ldg_256(reinterpret_cast<const float4*>(nodes_q) + 2 * (size_t) node, q0, q1);
+			ldg_32_bytes(reinterpret_cast<const float4*>(nodes_q) + 2 * (size_t) node, q0, q1);
 			const int ref0 = __float_as_int(q1.z), ref1 = __float_as_int(q1.w);
 			const bool h0 = ray_box_grid(__float_as_uint(q0.x), __float_as_uint(q0.y), __float_as_uint(q0.z), r, tmin, tmax, &tn0);
 			const bool h1 = ray_box_grid(__float_as_uint(q0.w), __float_as_uint(q1.x), __float_as_uint(q1.y), r, tmin, tmax, &tn1);
 #elif VKR_INTERLEAVED_NODES
-			// one interleaved pair (vkr_trace.cuh): the slab arithmetic of both children in packed FMAs
+			// one interleaved pair (vkr_trace.cuh): the slab arithmetic of both children side by side
 			const float4* nd = reinterpret_cast<const float4*>(reinterpret_cast<const char*>(nodes_i) + (size_t) ((uint32_t) node << 6));
 			float4 q0, q1, q2, q3;
-			ldg_256(nd, q0, q1); ldg_256(nd + 2, q2, q3);
+			ldg_32_bytes(nd, q0, q1); ldg_32_bytes(nd + 2, q2, q3);
 			const int ref0 = __float_as_int(q3.x), ref1 = __float_as_int(q3.y);
 			bool h0, h1;
 			{
@@ -513,7 +512,7 @@ VKR_DEV void trace_stream(const uint32_t base, const float4* __restrict__ nodes,
 			const float4* nd = nodes + 4 * (size_t) node;
 #endif
 			float4 q0, q1, q2, q3;
-			ldg_256(nd, q0, q1); ldg_256(nd + 2, q2, q3);
+			ldg_32_bytes(nd, q0, q1); ldg_32_bytes(nd + 2, q2, q3);
 			const int ref0 = __float_as_int(q3.x), ref1 = __float_as_int(q3.y);
 			const bool h0 = ray_box(q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, r, tmin, tmax, &tn0) && skip != 0;
 			const bool h1 = ray_box(q1.z, q1.w, q2.x, q2.y, q2.z, q2.w, r, tmin, tmax, &tn1) && skip != 1;

@@ -1,4 +1,4 @@
-// vkr_related_work.cuh -- the related-work polygon sampling techniques of the reference renderer for sm_100a
+// vkr_related_work.cuh -- the related-work polygon sampling techniques of the reference renderer for sm_90a
 // (SURVEY 8 row f4): the samplers the paper compares projected solid angle sampling against.
 //   src/shaders/polygon_sampling_related_work.glsl:38-1048  Turk (area), Urena (rectangle solid angle), Arvo (solid angle and
 //                                                           projected solid angle), Hart et al. (bilinear / biquadratic cosine warps)

@@ -1,4 +1,4 @@
-// vkr_related_work_kernel.cu -- the shading megakernel with the related-work polygon sampling techniques (sm_100a).
+// vkr_related_work_kernel.cu -- the shading megakernel with the related-work polygon sampling techniques (sm_90a).
 //
 // SURVEY 8 row f4: the samplers the reference compares projected solid angle sampling against (shading_pass.frag.glsl:332-481,
 // polygon_sampling_related_work.glsl): baseline, Turk, Urena, Arvo (solid angle / projected solid angle), solid angle with and

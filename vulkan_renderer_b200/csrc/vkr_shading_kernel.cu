@@ -1,4 +1,4 @@
-// vkr_shading_kernel.cu -- the per-screen-tile shading megakernel (sm_100a).
+// vkr_shading_kernel.cu -- the per-screen-tile shading megakernel (sm_90a).
 //
 // Replaces subpass 1 of the reference frame (src/main.c:1429-1434, the fragment shader
 // src/shaders/shading_pass.frag.glsl:824-866 with everything it calls). One CTA shades one

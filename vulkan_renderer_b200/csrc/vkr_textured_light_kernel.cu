@@ -1,4 +1,4 @@
-// vkr_textured_light_kernel.cu -- the shading megakernel for frames with textured polygonal lights (sm_100a).
+// vkr_textured_light_kernel.cu -- the shading megakernel for frames with textured polygonal lights (sm_90a).
 //
 // get_polygon_radiance() of the reference (src/shaders/shading_pass.frag.glsl:151-185) multiplies the light's radiance by a texture when its
 // texturing technique is not "none": an area texture in the light's plane, a light probe seen through the polygon (portal) or an IES profile,

@@ -1,4 +1,4 @@
-// vkr_textured_related_work_kernel.cu -- the related-work sampling techniques for frames with textured polygonal lights (sm_100a).
+// vkr_textured_related_work_kernel.cu -- the related-work sampling techniques for frames with textured polygonal lights (sm_90a).
 //
 // related_work_kernel (vkr_related_work_kernel.cu) with LIGHT_TEXTURES = true: the texture fetch of get_polygon_radiance()
 // (src/shaders/shading_pass.frag.glsl:151-185) where the shader has it, in the per-light code (vkr_related_work_light.cuh) and in the light

@@ -55,15 +55,10 @@ VKR_DEV bool ray_triangle(const float4* __restrict__ tri, f3 o, f3 d, float tmin
 	return true;
 }
 
-// One 32-byte half of a node with a single 256-bit load (LDG.E.256, sm_100): a node pair is two of these instead of three 128-bit and
-// one 64-bit load, which halves the wavefronts the L1 data pipe spends per visit -- the unit the trace warps keep busiest.
-VKR_DEV void ldg_256(const float4* __restrict__ p, float4& a, float4& b) {
-#if defined(__CUDA_ARCH__) && !defined(VKR_NO_LDG256)
-	asm("ld.global.nc.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-		: "=f"(a.x), "=f"(a.y), "=f"(a.z), "=f"(a.w), "=f"(b.x), "=f"(b.y), "=f"(b.z), "=f"(b.w) : "l"(p));
-#else
+// One 32-byte half of a node as two 128-bit loads through the read-only path (LDG.E.128.CONSTANT, the widest load sm_90 has): a node pair is
+// four of these, all of it in the two sectors of one 64-byte aligned pair.
+VKR_DEV void ldg_32_bytes(const float4* __restrict__ p, float4& a, float4& b) {
 	a = __ldg(p); b = __ldg(p + 1);
-#endif
 }
 
 // Reciprocal for the slab test only: the box test has to be conservative, not exact (header), so the hardware's approximation does (MUFU.RCP: relative
@@ -100,24 +95,17 @@ VKR_DEV bool ray_box(float cx, float cy, float cz, float hx, float hy, float hz,
 // ---------------------------------------------------------------------------------------------------------------------------------------
 // Interleaved node pairs: the same 64 bytes per pair with the two children's numbers next to each other,
 //   float 0..7   c0.x c1.x  c0.y c1.y  c0.z c1.z  h0.x h1.x        float 8..15   h0.y h1.y  h0.z h1.z  ref0 ref1  -  -
-// so that the two 256-bit loads of a visit leave (child 0, child 1) in aligned register pairs and the slab arithmetic of BOTH children is done by
-// the packed FMA of sm_100 (fma.rn.f32x2 -> FFMA2: pair * scalar + pair, the scalar broadcast with its sign / absolute value as operand modifiers):
-// 9 FFMA2 instead of 18 FFMA per visit, each half an IEEE fma with the operands of ray_box(), so a visit decides exactly as before. The trace warps are
-// bound by instruction issue (DESIGN.md section 3): a visit is ~50 instructions, every one taken out of it is worth 0.8 % of the frame.
+// so that the loads of a visit leave (child 0, child 1) side by side and the slab arithmetic of both children is one pairwise routine, ray_box_pair().
+// Each of its 18 FFMAs is an IEEE fma with the operands of ray_box(), so a visit decides exactly as with the plain pairs.
 VKR_DEV void interleave_node_pair(const float4* __restrict__ pair, float* out16) {
 	const float4 q0 = pair[0], q1 = pair[1], q2 = pair[2], q3 = pair[3];
 	out16[0] = q0.x; out16[1] = q1.z; out16[2] = q0.y; out16[3] = q1.w; out16[4] = q0.z; out16[5] = q2.x;   // centres
 	out16[6] = q0.w; out16[7] = q2.y; out16[8] = q1.x; out16[9] = q2.z; out16[10] = q1.y; out16[11] = q2.w; // half extents
 	out16[12] = q3.x; out16[13] = q3.y; out16[14] = 0.0f; out16[15] = 0.0f;
 }
-// (d0, d1) = (a0, a1) * s + (c0, c1), one instruction on the device
+// (d0, d1) = (a0, a1) * s + (c0, c1): two FFMAs (sm_90 has no packed fp32 FMA)
 VKR_DEV void fma_pair(float& d0, float& d1, float a0, float a1, float s, float c0, float c1) {
-#if defined(__CUDA_ARCH__)
-	asm("{ .reg .b64 a, b, c, d;\n\tmov.b64 a, {%2, %3};\n\tmov.b64 b, {%4, %4};\n\tmov.b64 c, {%5, %6};\n\tfma.rn.f32x2 d, a, b, c;\n\tmov.b64 {%0, %1}, d; }"
-		: "=f"(d0), "=f"(d1) : "f"(a0), "f"(a1), "f"(s), "f"(c0), "f"(c1));
-#else
 	d0 = fmaf(a0, s, c0); d1 = fmaf(a1, s, c1);
-#endif
 }
 // ray_box() for the two children of an interleaved pair (a = floats 0..7, b = floats 8..11)
 VKR_DEV void ray_box_pair(const float (&a)[8], const float (&b)[4], const ray_slabs& r, float tmin, float tmax, bool* h0, bool* h1, float* tn0, float* tn1) {
@@ -160,9 +148,8 @@ VKR_DEV bool occluded_interleaved(const float* __restrict__ pairs16, const float
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------------
-// Quantised node pairs: the form the trace warps of the shading kernels walk. ncu puts those warps at the limit of the L1 data pipe (74 % of its
-// wavefronts, 87 % of them node fetches of lanes that diverge): the lever is bytes per visit, not instructions. A pair shrinks from 64 to 32 bytes
-// -- one 256-bit load, one sector per lane -- by storing the two child boxes as 16-bit coordinates on a grid over the scene's bounding box:
+// Quantised node pairs: an edition of the trace warps' loop with half the bytes per visit (VKR_QUANTISED_NODES, vkr_ray_stream.cuh). A pair shrinks from
+// 64 to 32 bytes -- one sector per lane -- by storing the two child boxes as 16-bit coordinates on a grid over the scene's bounding box:
 //   word 0..2  child 0: x, y, z as (low | high << 16)      word 3..5  child 1      word 6, 7  the two child references (as in the float pairs)
 // Boxes are rounded outwards to the grid and one more cell (below), so the test stays conservative; the triangle predicate is untouched and hit / miss
 // remains the OR over the triangles it accepts. The ray is taken to grid coordinates once (t is invariant under per-axis scaling), a plane's
@@ -279,7 +266,7 @@ template <class Push>
 VKR_DEV int bvh4_descend_step(const float4* __restrict__ nodes4, int node, const ray_slabs& r, float tmin, float tmax, Push&& push) {
 	const float4* nd = nodes4 + 8 * (size_t) node;
 	float4 q0, q1, q2, q3, q4, q5, q6, q7;
-	ldg_256(nd, q0, q1); ldg_256(nd + 2, q2, q3); ldg_256(nd + 4, q4, q5); ldg_256(nd + 6, q6, q7);
+	ldg_32_bytes(nd, q0, q1); ldg_32_bytes(nd + 2, q2, q3); ldg_32_bytes(nd + 4, q4, q5); ldg_32_bytes(nd + 6, q6, q7);
 	const int ref0 = __float_as_int(q6.x), ref1 = __float_as_int(q6.y), ref2 = __float_as_int(q6.z), ref3 = __float_as_int(q6.w);
 	float tn0, tn1, tn2, tn3;
 	const bool h0 = ray_box(q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, r, tmin, tmax, &tn0);
