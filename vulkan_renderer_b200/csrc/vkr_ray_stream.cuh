@@ -358,7 +358,7 @@ VKR_DEV void trace_stream(const uint32_t base, const float4* __restrict__ nodes,
 #if VKR_QUANTISED_NODES
 	ray_grid r = make_ray_grid(make3(0.0f, 0.0f, 0.0f), make3(0.0f, 0.0f, 1.0f), grid_min, grid_scale);
 #else
-	ray_slabs r = make_slabs(make3(0.0f, 0.0f, 0.0f), make3(0.0f, 0.0f, 1.0f));
+	ray_slabs r = make_slabs<false>(make3(0.0f, 0.0f, 0.0f), make3(0.0f, 0.0f, 1.0f));
 #endif
 	while (true) {
 		// --- lanes whose ray has terminated draw a ticket and start on it as soon as it is published
@@ -419,7 +419,7 @@ VKR_DEV void trace_stream(const uint32_t base, const float4* __restrict__ nodes,
 #if VKR_QUANTISED_NODES
 							r = make_ray_grid(o, d, grid_min, grid_scale);
 #else
-							r = make_slabs(o, d);
+							r = make_slabs<false>(o, d);   // shading rays: no direction component below 2^-64 but zero (vkr_trace.cuh)
 #endif
 							top = stack_bottom; push(kTraversalDone);
 #if VKR_ANCHORED

@@ -64,19 +64,30 @@ VKR_DEV void ldg_32_bytes(const float4* __restrict__ p, float4& a, float4& b) {
 // Reciprocal for the slab test only: the box test has to be conservative, not exact (header), so the hardware's approximation does (MUFU.RCP: relative
 // error 2^-23, i.e. one more rounding of the size the padding of the boxes is made for; denormal components flush to zero, whose reciprocal is infinite,
 // and an infinite or NaN slab distance leaves the slab unconstrained). Saves three IEEE divisions (range check, refinement, slow path) per ray set-up.
-VKR_DEV float slab_reciprocal(float x) {
+VKR_DEV float unguarded_slab_reciprocal(float x) {
 #if defined(__CUDA_ARCH__) && !defined(VKR_EXACT_SLAB_RECIPROCAL)
 	float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y;
 #else
 	return 1.0f / x;
 #endif
 }
+// Components below 2^-64 in magnitude get an infinite reciprocal too, which drops that axis from the test (always conservative). A finite but huge
+// reciprocal (1/FLT_MIN = 2^126) makes o / d overflow to infinity while c / d - o / d is finite, and the slab test culls boxes the ray crosses.
+// With |id| <= 2^64 no product or fma of the slab test overflows for coordinates below 2^60.
+VKR_DEV float slab_reciprocal(float x) {
+	const float y = unguarded_slab_reciprocal(x);
+	return (fabsf(x) < 5.421010862427522e-20f) ? copysignf(__int_as_float(0x7f800000), x) : y;   // 2^-64
+}
 
-// Ray in the form the slab test wants: id = 1/d, oid = o/d
+// Ray in the form the slab test wants: id = 1/d, oid = o/d. GUARDED = false is for the trace warps of the shading kernel only (vkr_ray_stream.cuh),
+// which stay instruction for instruction as they were: their rays point from a surface point to a point on a light, normalised, so a nonzero
+// component is far above 2^-64 for any scene with coordinates above 1e-12.
 struct ray_slabs { f3 id, oid; };
+template <bool GUARDED = true>
 VKR_DEV ray_slabs make_slabs(f3 o, f3 d) {
 	ray_slabs r;
-	r.id = make3(slab_reciprocal(d.x), slab_reciprocal(d.y), slab_reciprocal(d.z));
+	if (GUARDED) r.id = make3(slab_reciprocal(d.x), slab_reciprocal(d.y), slab_reciprocal(d.z));
+	else r.id = make3(unguarded_slab_reciprocal(d.x), unguarded_slab_reciprocal(d.y), unguarded_slab_reciprocal(d.z));
 	r.oid = make3(o.x * r.id.x, o.y * r.id.y, o.z * r.id.z);
 	return r;
 }
