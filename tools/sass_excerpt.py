@@ -5,7 +5,7 @@
 
 shading_kernel<3,5,0,0,1> (quad lights, diffuse + specular MIS, shadow rays) from the in-tree object: resource usage, the instruction mix, the bulk copy of
 the constant block (UBLKCP) with its mbarrier, the register hand-over between trace and shading warps (USETMAXREG) and the trace warps' node loop
-(two 256-bit node fetches, the slab test on the FMA pipe, FMNMX3)."""
+(four 128-bit node fetches, the slab test on the FMA pipe, its min / max as VIMNMX3 + VIMNMX)."""
 import collections
 import os
 import re
@@ -29,8 +29,8 @@ def main():
 	out = ["# SASS of `shading_kernel<3,5,0,0,1>` (sm_90a), commit %s" % git, "",
 		"`cuobjdump -sass -fun %s vulkan_renderer_b200/build/vkr_shading_kernel_maxp5.cu.o`, excerpts." % KERNEL, "",
 		"* resource usage: `%s`" % (usage[0] if usage else "?"),
-		"* %d instructions; FFMA / FMUL / FADD %d, FMNMX %d, MUFU %d, LDG %d (of them 128-bit: %d), LDS / STS %d, LDL / STL (spills) %d, VOTE / SHFL %d" % (
-			len(lines), family({"FFMA", "FMUL", "FADD"}), family({"FMNMX"}), family({"MUFU"}), family({"LDG"}), sum(v for k, v in ops.items() if k.startswith("LDG") and ".128" in k),
+		"* %d instructions; FFMA / FMUL / FADD %d, FMNMX %d, VIMNMX3 / VIMNMX %d, MUFU %d, LDG %d (of them 128-bit: %d), LDS / STS %d, LDL / STL (spills) %d, VOTE / SHFL %d" % (
+			len(lines), family({"FFMA", "FMUL", "FADD"}), family({"FMNMX"}), family({"VIMNMX3", "VIMNMX"}), family({"MUFU"}), family({"LDG"}), sum(v for k, v in ops.items() if k.startswith("LDG") and ".128" in k),
 			family({"LDS", "STS"}), family({"LDL", "STL"}), family({"VOTE", "VOTEU", "SHFL"})),
 		"* no tensor-core or tensor-map instructions (HMMA / HGMMA / UTMALDG count: %d): the path has no contraction" % family({"HMMA", "HGMMA", "UTMALDG"}), ""]
 	def excerpt(title, pattern, before, after, limit=1):
@@ -39,7 +39,7 @@ def main():
 			out.extend(["## %s" % title, "", "```"] + lines[max(0, i - before):i + after + 1] + ["```", ""])
 	excerpt("Constant block: one bulk asynchronous copy into shared memory, completion on an mbarrier", r"UBLKCP", 6, 8)
 	excerpt("Role split: trace warps give registers to the shading warps", r"USETMAXREG", 2, 3, limit=2)
-	excerpt("Trace warps: the node loop (one node pair = four 128-bit loads; slab test as FFMA + FMNMX; shared-memory stack)", r"LDG\.E\.128\.CONSTANT", 4, 62)
+	excerpt("Trace warps: the node loop (one node pair = four 128-bit loads; slab test as FFMA + VIMNMX3 / VIMNMX; shared-memory stack)", r"VIMNMX3", 40, 40)
 	excerpt("Trace warps: ticket draw (one shared-memory atomic per warp refill)", r"ATOMS\.ADD", 8, 6)
 	path = os.path.join(ROOT, "profiles", "%s_sass_excerpt.md" % tag)
 	os.makedirs(os.path.dirname(path), exist_ok=True)

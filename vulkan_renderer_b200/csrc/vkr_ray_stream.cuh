@@ -41,8 +41,10 @@ constexpr unsigned kPending = 0xffu;
 #ifndef VKR_BVH_WIDTH
 #define VKR_BVH_WIDTH 2   // children per node of the shadow BVH the trace warps walk; 4 = experimental variant (see trace_stream)
 #endif
+// The node loop is left once fewer than this many lanes of a trace warp descend (lane utilisation only, never results). On an H100 (400 W) the C3 frame
+// took 381.4 / 381.5 ms with 8, 388.6 / 391.2 ms with 16 and 442.7 / 443.1 ms with 24 (second frame of two alternating runs each, same frame hash).
 #ifndef VKR_NODE_LOOP_MIN_LANES
-#define VKR_NODE_LOOP_MIN_LANES 16
+#define VKR_NODE_LOOP_MIN_LANES 8
 #endif
 constexpr int kNodeLoopMinLanes = VKR_NODE_LOOP_MIN_LANES;
 // Tuning knobs of the trace warps' round (lane utilisation only, never results): a new batch of rays is set up once at least VKR_REFILL_MIN_LANES lanes are
@@ -418,6 +420,8 @@ VKR_DEV void trace_stream(const uint32_t base, const float4* __restrict__ nodes,
 						else {
 #if VKR_QUANTISED_NODES
 							r = make_ray_grid(o, d, grid_min, grid_scale);
+#elif VKR_INTERLEAVED_NODES
+							r = make_clamped_slabs(o, d);   // no NaN slab distance: the integer min / max of ray_box_pair<true> (vkr_trace.cuh)
 #else
 							r = make_slabs<false>(o, d);   // shading rays: no direction component below 2^-64 but zero (vkr_trace.cuh)
 #endif
@@ -481,7 +485,7 @@ VKR_DEV void trace_stream(const uint32_t base, const float4* __restrict__ nodes,
 				VKR_STAT(st_siblings);
 			}
 #else
-		while (node >= 0 && node != kTraversalDone) {
+		while ((unsigned) node < (unsigned) kTraversalDone) {   // node >= 0 && node != kTraversalDone, one compare
 			const int skip = 2;
 #endif
 			float tn0, tn1;
@@ -502,7 +506,7 @@ VKR_DEV void trace_stream(const uint32_t base, const float4* __restrict__ nodes,
 			bool h0, h1;
 			{
 				const float a[8] = { q0.x, q0.y, q0.z, q0.w, q1.x, q1.y, q1.z, q1.w }, b[4] = { q2.x, q2.y, q2.z, q2.w };
-				ray_box_pair(a, b, r, tmin, tmax, &h0, &h1, &tn0, &tn1);
+				ray_box_pair<true>(a, b, r, tmin, tmax, &h0, &h1, &tn0, &tn1);   // 0 < tmin < tmax: rays with tmax <= tmin never start
 			}
 #else
 #if VKR_LEAN_NODE_STEP

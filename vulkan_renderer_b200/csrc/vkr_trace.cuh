@@ -19,6 +19,12 @@
 // and no per-axis min/max, which moves the work from the ALU pipe (FMNMX, the busiest pipe of the
 // traversal loop) to the FMA pipe. Its rounding error is below 1/64 of the padding the builder adds
 // to every box (vkr_bvh.cpp), so no triangle the predicate accepts is culled.
+// The shading kernel's trace warps (ray_box_pair<true>) take the max of the near and the min of the far
+// distances as signed integers on the float bits (sm_90 DPX: VIMNMX3). That is exact for 0 < tmin < tmax
+// and slab distances that are never NaN, which the set-up guarantees by clamping the reciprocal to +-2^64
+// (make_clamped_slabs): with |id| <= 2^64, c*id - o*id is finite for coordinates below 2^60 and its
+// rounding stays the few ulp the padding covers; a zero component then tests the origin against that
+// axis's slab instead of dropping the axis.
 #pragma once
 #include "vkr_device_math.cuh"
 
@@ -79,9 +85,9 @@ VKR_DEV float slab_reciprocal(float x) {
 	return (fabsf(x) < 5.421010862427522e-20f) ? copysignf(__int_as_float(0x7f800000), x) : y;   // 2^-64
 }
 
-// Ray in the form the slab test wants: id = 1/d, oid = o/d. GUARDED = false is for the trace warps of the shading kernel only (vkr_ray_stream.cuh),
-// which stay instruction for instruction as they were: their rays point from a surface point to a point on a light, normalised, so a nonzero
-// component is far above 2^-64 for any scene with coordinates above 1e-12.
+// Ray in the form the slab test wants: id = 1/d, oid = o/d. GUARDED = false is for the compile-time editions of the trace warps' loop
+// (vkr_ray_stream.cuh): their rays point from a surface point to a point on a light, normalised, so a nonzero component is far above 2^-64 for any
+// scene with coordinates above 1e-12.
 struct ray_slabs { f3 id, oid; };
 template <bool GUARDED = true>
 VKR_DEV ray_slabs make_slabs(f3 o, f3 d) {
@@ -91,6 +97,42 @@ VKR_DEV ray_slabs make_slabs(f3 o, f3 d) {
 	r.oid = make3(o.x * r.id.x, o.y * r.id.y, o.z * r.id.z);
 	return r;
 }
+// Set-up for the integer min / max of ray_box_pair<true>: the reciprocal clamped to [-2^64, 2^64] (zero and denormal components get +-2^64 with
+// their sign, a NaN component -2^64), so every slab distance is finite or +-infinity and never NaN: with finite operands neither o * id nor an fma of
+// the slab test can be NaN, an overflow only saturates. For coordinates below 2^60 in magnitude nothing overflows (2^60 * 2^64 = 2^124), and the
+// rounding of c * id - o * id is a few ulp of the coordinates, the same error the unclamped test has (header). The clamp is conservative: an axis whose
+// component is below 2^-64 keeps the slab [(c - h - o) * 2^64, (c + h - o) * 2^64] (times the sign). A triangle in the box hit at distance t lies at
+// least the padding (2^-16 of the scene extent) inside the slab, and the ray moves less than t * 2^-64 along that axis, so the slab reaches from below
+// -(pad - t 2^-64) 2^64 < 0 to above (pad - t 2^-64) 2^64 > t as long as t < pad * 2^63 -- 2^47 scene extents. Exactly zero components, which the
+// unclamped test drops from the test (NaN slab distances), now test the origin against the slab, so such rays may visit fewer pairs; their answers stay.
+VKR_DEV float clamped_slab_reciprocal(float x) {
+	const float big = 18446744073709551616.0f;   // 2^64
+	return fminf(fmaxf(unguarded_slab_reciprocal(x), -big), big);
+}
+VKR_DEV ray_slabs make_clamped_slabs(f3 o, f3 d) {
+	ray_slabs r;
+	r.id = make3(clamped_slab_reciprocal(d.x), clamped_slab_reciprocal(d.y), clamped_slab_reciprocal(d.z));
+	r.oid = make3(o.x * r.id.x, o.y * r.id.y, o.z * r.id.z);
+	return r;
+}
+
+// Signed 32-bit max / min of three (sm_90 DPX: one VIMNMX3) and of two. The host build of this header runs the same integer semantics.
+VKR_DEV int imax3_s32(int a, int b, int c) {
+#if defined(__CUDA_ARCH__)
+	return __vimax3_s32(a, b, c);
+#else
+	const int m = (a > b) ? a : b; return (m > c) ? m : c;
+#endif
+}
+VKR_DEV int imin3_s32(int a, int b, int c) {
+#if defined(__CUDA_ARCH__)
+	return __vimin3_s32(a, b, c);
+#else
+	const int m = (a < b) ? a : b; return (m < c) ? m : c;
+#endif
+}
+VKR_DEV int imax_s32(int a, int b) { return (a > b) ? a : b; }
+VKR_DEV int imin_s32(int a, int b) { return (a < b) ? a : b; }
 
 // Conservative slab test (see header) of the box with centre c and half extent h. Returns the entry distance in
 // *t_near. NaNs (inf - inf for axis-parallel rays) drop out of fminf/fmaxf, which leaves that slab unconstrained.
@@ -119,6 +161,12 @@ VKR_DEV void fma_pair(float& d0, float& d1, float a0, float a1, float s, float c
 	d0 = fmaf(a0, s, c0); d1 = fmaf(a1, s, c1);
 }
 // ray_box() for the two children of an interleaved pair (a = floats 0..7, b = floats 8..11)
+// DPX = true (the trace warps of the shading kernel): near and far distances are combined as signed integers on the float bits, one VIMNMX3 + one
+// VIMNMX per child and side instead of three FMNMX. That gives fmaxf / fminf's answers when (1) no distance is NaN -- the slabs come from
+// make_clamped_slabs() -- and (2) 0 < tmin < tmax: the max then includes the positive tmin, and positive floats order like their bits as integers, so
+// tn is exactly fmaxf's; if a far distance is negative (or -0) the integer min is some negative value (or -0) where fminf's is the most negative one,
+// and both fail tn <= tf; otherwise all far distances are positive and the min is exact. The order of two hit children compares two positive tn.
+template <bool DPX = false>
 VKR_DEV void ray_box_pair(const float (&a)[8], const float (&b)[4], const ray_slabs& r, float tmin, float tmax, bool* h0, bool* h1, float* tn0, float* tn1) {
 	float mx0, mx1, my0, my1, mz0, mz1, nx0, nx1, ny0, ny1, nz0, nz1, fx0, fx1, fy0, fy1, fz0, fz1;
 	const float nox = -r.oid.x, noy = -r.oid.y, noz = -r.oid.z;
@@ -126,14 +174,26 @@ VKR_DEV void ray_box_pair(const float (&a)[8], const float (&b)[4], const ray_sl
 	const float ax = fabsf(r.id.x), ay = fabsf(r.id.y), az = fabsf(r.id.z);
 	fma_pair(nx0, nx1, a[6], a[7], -ax, mx0, mx1); fma_pair(ny0, ny1, b[0], b[1], -ay, my0, my1); fma_pair(nz0, nz1, b[2], b[3], -az, mz0, mz1);
 	fma_pair(fx0, fx1, a[6], a[7], ax, mx0, mx1); fma_pair(fy0, fy1, b[0], b[1], ay, my0, my1); fma_pair(fz0, fz1, b[2], b[3], az, mz0, mz1);
-	*tn0 = fmaxf(fmaxf(nx0, ny0), fmaxf(nz0, tmin)); *tn1 = fmaxf(fmaxf(nx1, ny1), fmaxf(nz1, tmin));
-	const float tf0 = fminf(fminf(fx0, fy0), fminf(fz0, tmax)), tf1 = fminf(fminf(fx1, fy1), fminf(fz1, tmax));
+	float tf0, tf1;
+	if (DPX) {
+		const int lo = __float_as_int(tmin), hi = __float_as_int(tmax);
+		*tn0 = __int_as_float(imax_s32(imax3_s32(__float_as_int(nx0), __float_as_int(ny0), __float_as_int(nz0)), lo));
+		*tn1 = __int_as_float(imax_s32(imax3_s32(__float_as_int(nx1), __float_as_int(ny1), __float_as_int(nz1)), lo));
+		tf0 = __int_as_float(imin_s32(imin3_s32(__float_as_int(fx0), __float_as_int(fy0), __float_as_int(fz0)), hi));
+		tf1 = __int_as_float(imin_s32(imin3_s32(__float_as_int(fx1), __float_as_int(fy1), __float_as_int(fz1)), hi));
+	}
+	else {
+		*tn0 = fmaxf(fmaxf(nx0, ny0), fmaxf(nz0, tmin)); *tn1 = fmaxf(fmaxf(nx1, ny1), fmaxf(nz1, tmin));
+		tf0 = fminf(fminf(fx0, fy0), fminf(fz0, tmax)); tf1 = fminf(fminf(fx1, fy1), fminf(fz1, tmax));
+	}
 	*h0 = *tn0 <= tf0; *h1 = *tn1 <= tf1;
 }
 // Per-thread any-hit query over interleaved pairs (16 floats each): the reference form of the trace warps' loop, run on the CPU against occluded().
+// DPX = true is the form the shading kernel runs (clamped set-up, integer min / max); false the fmaxf form with the guarded set-up.
+template <bool DPX = false>
 VKR_DEV bool occluded_interleaved(const float* __restrict__ pairs16, const float4* __restrict__ tris, f3 o, f3 d, float tmin, float tmax, int* stack, int stride, int* visits) {
 	if (!(tmax > tmin)) return false;
-	const ray_slabs r = make_slabs(o, d);
+	const ray_slabs r = DPX ? make_clamped_slabs(o, d) : make_slabs(o, d);
 	int sp = 0, node = 0;
 	float t, tn0, tn1;
 	while (true) {
@@ -149,7 +209,7 @@ VKR_DEV bool occluded_interleaved(const float* __restrict__ pairs16, const float
 		const float* w = pairs16 + 16 * (size_t) node;
 		const float a[8] = { w[0], w[1], w[2], w[3], w[4], w[5], w[6], w[7] }, b[4] = { w[8], w[9], w[10], w[11] };
 		bool h0, h1;
-		ray_box_pair(a, b, r, tmin, tmax, &h0, &h1, &tn0, &tn1);
+		ray_box_pair<DPX>(a, b, r, tmin, tmax, &h0, &h1, &tn0, &tn1);
 		const int ref0 = __float_as_int(w[12]), ref1 = __float_as_int(w[13]);
 		if (h0 && h1) { const bool swap = tn1 < tn0; stack[sp * stride] = swap ? ref0 : ref1; ++sp; node = swap ? ref1 : ref0; }
 		else if (h0) node = ref0;
