@@ -450,6 +450,42 @@ void vkr_record_frame_time(double time_in_seconds);
 float vkr_get_frame_time(void);
 void vkr_reset_frame_times(void);
 
+/* ---- averaging frames and measuring their error (no counterpart in the reference, which shows one frame at a time). What is accumulated is the
+        frame as the shading pass stores it: linear radiance times the exposure factor, RGB; alpha is ignored. A pixel whose radiance was NaN has been
+        painted pink by the pass (as the reference does), so it counts as that colour. Accumulate frames of a pass with output_srgb = 0 and
+        g_frame_bits = 0 (vkr_set_frame_bits); sRGB or half-bit frames are not radiance. Frames of independent noise come from animate_noise = 1 in
+        the render settings: each vkr_write_constants() call then draws new random numbers.
+        All arithmetic is float64 and every sum has a fixed order (csrc/vkr_accumulate.cuh), so results are bit-identical from call to call and from
+        device to device. Asynchronous on device->stream unless marked synchronous; those wait for device->stream only. */
+typedef struct vkr_accumulator_s {
+	uint32_t width, height;
+	uint64_t frame_count;   /* frames added since create / reset */
+	void* d_state;          /* 6 planes of width*height double: mean rgb, m2 rgb (Welford) */
+	void* d_partials; void* h_partials;   /* reduction scratch, pinned host copy */
+} vkr_accumulator_t;
+/* 48 bytes of state per pixel (99.5 MB at 1920x1080) */
+int vkr_create_accumulator(vkr_accumulator_t* accumulator, const vkr_device_t* device, uint32_t width, uint32_t height);
+void vkr_destroy_accumulator(vkr_accumulator_t* accumulator, const vkr_device_t* device);
+/* frame_count = 0; the next frame replaces the state */
+int vkr_accumulator_reset(vkr_accumulator_t* accumulator, const vkr_device_t* device);
+/* d_frame_rgba32f: DEVICE pointer, width*height float4 (16-byte aligned), e.g. vkr_render_targets_t::d_frame after vkr_shading_pass_run. Per pixel and
+   channel, frame n = frame_count + 1: d = x - mean; mean += d / n; m2 += d * (x - mean) (the first frame is stored as it is) */
+int vkr_accumulate_frame(vkr_accumulator_t* accumulator, const vkr_device_t* device, const void* d_frame_rgba32f);
+/* DEVICE pointers, width*height float4 each, either may be NULL: the mean rounded to float (alpha 1) and the per-frame sample variance
+   m2 / (frame_count - 1) rounded to float (alpha 0). Refuses frame_count == 0, and a variance with frame_count < 2. */
+int vkr_accumulator_resolve(const vkr_accumulator_t* accumulator, const vkr_device_t* device, void* d_mean_rgba32f, void* d_variance_rgba32f);
+/* synchronous: per channel, the mean over all pixels of the per-frame sample variance -- the noise level of a setting, no reference needed. frame_count >= 2. */
+int vkr_accumulator_mean_variance(const vkr_accumulator_t* accumulator, const vkr_device_t* device, double out_mean_variance[3]);
+/* A frame x against a reference r, over the pixels whose six RGB inputs are finite (N = pixel_count), in float64 from the exactly converted floats:
+   mse[c] = sum (x-r)^2 / N; rel_mse[c] = sum (x-r)^2 / (r^2 + 0.01) / N; mae[c] = sum |x-r| / N; max_abs_error over all channels. The means are
+   NaN if N = 0. nonfinite_pixels: pixels left out. */
+typedef struct vkr_frame_error_s {
+	double mse[3], rel_mse[3], mae[3], max_abs_error;
+	uint64_t pixel_count, nonfinite_pixels;
+} vkr_frame_error_t;
+/* synchronous; both frames are DEVICE pointers to width*height float4 */
+int vkr_compare_frames(const vkr_device_t* device, uint32_t width, uint32_t height, const void* d_frame_rgba32f, const void* d_reference_rgba32f, vkr_frame_error_t* out);
+
 /* ---- shadow-ray probe (tests / KATs): rays = {ox,oy,oz,dx,dy,dz,tmin,tmax} per ray on the HOST, out = 1 byte per ray */
 int vkr_trace_shadow_rays(const vkr_device_t* device, const vkr_scene_t* scene, uint32_t ray_count, const float* rays, uint8_t* out_occluded);
 /* ---- sampling probe (tests / KATs): clip + prepare + sample in the polygon's local space on the device */

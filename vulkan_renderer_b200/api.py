@@ -27,6 +27,7 @@ EXPORTED_SYMBOLS = [
 	"vkr_record_frame_time", "vkr_get_frame_time", "vkr_reset_frame_times",
 	"vkr_load_texture", "vkr_destroy_texture", "vkr_texture_from_levels", "vkr_scene_from_buffers", "vkr_ltc_table_from_images", "vkr_noise_table_from_image", "vkr_create_and_assign_light_textures", "vkr_destroy_light_textures",
 	"vkr_create_render_targets", "vkr_destroy_render_targets", "vkr_download_frame", "vkr_download_gbuffer", "vkr_upload_gbuffer",
+	"vkr_create_accumulator", "vkr_destroy_accumulator", "vkr_accumulator_reset", "vkr_accumulate_frame", "vkr_accumulator_resolve", "vkr_accumulator_mean_variance", "vkr_compare_frames",
 ]
 
 # enums (values = the reference's)
@@ -137,6 +138,17 @@ class FrameExchange(C.Structure):
 		("d_peer_blocks", C.c_void_p * MAX_GPUS), ("peer_is_ipc", C.c_int * MAX_GPUS), ("frames_exchanged", C.c_uint64), ("h_status", C.POINTER(C.c_int)), ("timeout_ns", C.c_uint64)]
 
 
+class Accumulator(C.Structure):
+	"""vkr_accumulator_t: running mean and sum of squared deviations of frames, float64 (include/vkr_b200.h)."""
+	_fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("frame_count", C.c_uint64), ("d_state", C.c_void_p), ("d_partials", C.c_void_p), ("h_partials", C.c_void_p)]
+
+
+class FrameError(C.Structure):
+	"""vkr_frame_error_t: a frame against a reference over the pixels with finite inputs."""
+	_fields_ = [("mse", C.c_double * 3), ("rel_mse", C.c_double * 3), ("mae", C.c_double * 3), ("max_abs_error", C.c_double),
+		("pixel_count", C.c_uint64), ("nonfinite_pixels", C.c_uint64)]
+
+
 TRACE_COUNTER_NAMES = ["rays", "occluded", "cache_hits", "node_visits", "leaf_visits", "triangle_tests", "warp_rounds", "warp_node_steps", "known_occluded", "idle_polls",
 	"entries", "resolve_polls", "candidates"]   # vkr_trace_counter_t
 TRACE_COUNTER_COUNT = 16
@@ -223,5 +235,12 @@ def load_library():
 	lib.vkr_record_frame_time.argtypes = [C.c_double]; lib.vkr_record_frame_time.restype = None
 	lib.vkr_get_frame_time.argtypes = []; lib.vkr_get_frame_time.restype = C.c_float
 	lib.vkr_reset_frame_times.argtypes = []; lib.vkr_reset_frame_times.restype = None
+	lib.vkr_create_accumulator.argtypes = [P(Accumulator), P(Device), C.c_uint32, C.c_uint32]
+	lib.vkr_destroy_accumulator.argtypes = [P(Accumulator), P(Device)]; lib.vkr_destroy_accumulator.restype = None
+	lib.vkr_accumulator_reset.argtypes = [P(Accumulator), P(Device)]
+	lib.vkr_accumulate_frame.argtypes = [P(Accumulator), P(Device), C.c_void_p]
+	lib.vkr_accumulator_resolve.argtypes = [P(Accumulator), P(Device), C.c_void_p, C.c_void_p]
+	lib.vkr_accumulator_mean_variance.argtypes = [P(Accumulator), P(Device), P(C.c_double)]
+	lib.vkr_compare_frames.argtypes = [P(Device), C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, P(FrameError)]
 	_lib = lib
 	return lib

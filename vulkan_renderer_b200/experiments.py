@@ -12,7 +12,8 @@ file name (advance_experiments, src/main.c:1948-2016; get_frame_time, src/frame_
 
 on the synthetic stand-ins of the scenes (vulkan_renderer_b200.synth; the reference's assets are not in its repository) and
 runs them through the C-ABI: one shading pass per experiment, frame time = the median of the recorded frame times, kernel
-times from CUDA events. Output: one JSON record per experiment and, optionally, the screenshot (*.png or *.hdr).
+times from CUDA events. Output: one JSON record per experiment and, optionally, the screenshot (*.png or *.hdr). convergence_groups() and
+run_convergence() measure the figures' error against converged references and their noise (vulkan_renderer_b200.convergence).
 Everything that computes goes through libvkr_b200.so; there is no CPU fallback.
 """
 import ctypes as C
@@ -152,6 +153,17 @@ def prepare_data(experiment, data_root):
 	return synth.build_dataset(os.path.join(data_root, tag), experiment["scene"], **experiment["scene_parameters"])
 
 
+def _configure(frame, experiment):
+	"""Applies an experiment's render settings and light count to a Frame."""
+	for key, value in experiment["settings"].items():
+		if key == "error_display":
+			frame.configure(error_display=value)   # a pass setting (-D defines), not part of the constant block
+		else:
+			setattr(frame.settings, key, value)
+	if experiment.get("light_count"):
+		frame.configure(light_count=experiment["light_count"])
+
+
 def run_experiment(experiment, data_root, out_dir=None, frames=12, warmup=3, width=None, height=None, cuda_device=0, screenshot=True):
 	"""Runs one experiment like the application does: set up scene, lights and settings, render `warmup` + `frames` frames, take the
 	median frame time, store the screenshot under its path with the time in milliseconds filled in. Returns the JSON record."""
@@ -165,13 +177,7 @@ def run_experiment(experiment, data_root, out_dir=None, frames=12, warmup=3, wid
 	targets = api.RenderTargets()
 	try:
 		s = experiment["settings"]
-		for key, value in s.items():
-			if key == "error_display":
-				frame.configure(error_display=value)   # a pass setting (-D defines), not part of the constant block
-			else:
-				setattr(frame.settings, key, value)
-		if experiment.get("light_count"):
-			frame.configure(light_count=experiment["light_count"])
+		_configure(frame, experiment)
 		constants = frame.constants(width, height)
 		frame._check(lib.vkr_create_render_targets(C.byref(targets), C.byref(frame.device), width, height), "vkr_create_render_targets")
 		frame._check(lib.vkr_run_visibility_pass(C.byref(frame.device), C.byref(frame.scene), constants, width, height, targets.d_visibility), "vkr_run_visibility_pass")
@@ -215,4 +221,94 @@ def run(experiments, data_root, out_dir, json_path=None, **kw):
 		os.makedirs(os.path.dirname(os.path.abspath(json_path)), exist_ok=True)
 		with open(json_path, "w") as f:
 			json.dump(records, f, indent=1)
+	return records
+
+
+def convergence_groups():
+	"""The figure experiments whose error can be measured, each with the experiment of the list that serves as its reference: same scene, scene
+	parameters, quicksave, resolution, exposure and light display. Left out: the error displays (they show no radiance) and the figures without a
+	reference of their own view (the IES profile attic, the textured screen)."""
+	names = [e["name"] for e in experiment_list(all_timings=False)]
+	def members(prefix, reference, exclude=()):
+		return [n for n in names if n.startswith(prefix) and n != reference and n not in exclude]
+	cornell_tilted = "cornell_box_projected_solid_angle_arvo_tilted_1spp"
+	return [
+		dict(name="attic", reference="attic_reference_128spp", members=members("attic_", "attic_reference_128spp")),
+		dict(name="bistro_small", reference="bistro_small_polygon_reference_128spp", members=members("bistro_small_", "bistro_small_polygon_reference_128spp")),
+		dict(name="bistro_tiny", reference="bistro_tiny_polygon_reference_128spp", members=members("bistro_tiny_", "bistro_tiny_polygon_reference_128spp")),
+		dict(name="mis_plane", reference="mis_plane_reference_128spp", members=members("mis_plane_", "mis_plane_reference_128spp")),
+		dict(name="cornell_box", reference="cornell_box_reference_128spp", members=members("cornell_box_", "cornell_box_reference_128spp", (cornell_tilted, "cornell_box_reference_tilted_128spp"))),
+		dict(name="cornell_box_tilted", reference="cornell_box_reference_tilted_128spp", members=[cornell_tilted]),
+		dict(name="shadowed_plane", reference="shadowed_plane_reference_4096spp", members=["shadowed_plane_biased_4096spp"]),   # the bias test
+		dict(name="roughness_planes", reference="roughness_planes_lambertian_2spp", members=["roughness_planes_lambertian_diffuse_only_1spp"]),
+	]
+
+
+def run_convergence(group, data_root, out_dir, reference_frames, variance_frames, width=None, height=None, cuda_device=0):
+	"""Measures the members of one convergence group (convergence_groups()) against a converged reference: the reference experiment's settings
+	averaged over `reference_frames` animated frames. Per member: its screenshot frame (animate_noise = 0, the frame run_experiment shades, in linear
+	radiance) against that reference, and the mean per-frame variance over `variance_frames` animated frames. The record also holds the error of the
+	reference experiment's own screenshot frame (reference_frame_error). With out_dir, the reference is stored as out_dir/convergence/<group>_reference.hdr.
+	Returns the JSON record."""
+	from . import convergence
+	from .frame import Frame
+	by_name = {e["name"]: e for e in experiment_list(all_timings=False)}
+
+	def open_frame(experiment):
+		info = prepare_data(experiment, data_root)
+		frame = Frame(info["vks"], info["textures"], info["save"], info["ltc"], cuda_device=cuda_device)
+		_configure(frame, experiment)
+		return frame
+
+	ref_experiment = by_name[group["reference"]]
+	w = width or ref_experiment["width"]; h = height or ref_experiment["height"]
+	frame = open_frame(ref_experiment)
+	try:
+		reference = convergence.accumulate(frame, w, h, reference_frames, animate=True)
+		# the reference experiment's own screenshot frame against the converged image: the error of one frame of these settings (for the bias test: unbiased)
+		reference_frame_error = convergence.frame_error(frame, convergence.accumulate(frame, w, h, 1, animate=False).mean, reference.mean)
+		if out_dir is not None:
+			path = os.path.join(out_dir, "convergence", "%s_reference.hdr" % group["name"])
+			os.makedirs(os.path.dirname(path), exist_ok=True)
+			rgb = reference.mean[..., :3].copy()
+			frame._check(frame.lib.vkr_write_hdr(path.encode(), w, h, rgb.ctypes.data), "vkr_write_hdr")
+	finally:
+		frame.close()
+	record = dict(group=group["name"], reference=group["reference"], width=w, height=h, reference_frames=reference_frames,
+		reference_samples_per_pixel=ref_experiment["settings"]["sample_count"] * reference_frames,
+		reference_mean_variance=list(reference.mean_variance) if reference.mean_variance is not None else None,
+		reference_frame_error=reference_frame_error, accumulate_ms_per_frame=round(reference.accumulate_ms_per_frame, 5), variance_frames=variance_frames,
+		timed="accumulate kernel per frame at %dx%d, CUDA events" % (w, h), members=[])
+	for name in group["members"]:
+		experiment = by_name[name]
+		frame = open_frame(experiment)
+		try:
+			screenshot = convergence.accumulate(frame, w, h, 1, animate=False).mean
+			error = convergence.frame_error(frame, screenshot, reference.mean)
+			noise = convergence.accumulate(frame, w, h, variance_frames, animate=True) if variance_frames >= 2 else None
+		finally:
+			frame.close()
+		member = dict(name=name, settings=dict(experiment["settings"]), samples_per_pixel=experiment["settings"]["sample_count"],
+			mse=error["mse"], rel_mse=error["rel_mse"], mae=error["mae"], max_abs_error=error["max_abs_error"], nonfinite_pixels=error["nonfinite_pixels"],
+			mean_variance=list(noise.mean_variance) if noise is not None else None)
+		record["members"].append(member)
+	return record
+
+
+def run_convergences(groups, data_root, out_dir, json_path, reference_frames, variance_frames, **kw):
+	"""Runs the groups in order and writes their records as JSON (a list, see run_convergence)."""
+	records = []
+	for group in groups:
+		record = run_convergence(group, data_root, out_dir, reference_frames, variance_frames, **kw)
+		records.append(record)
+		print("%s against %s (%d frames, %dx%d; accumulate %.4f ms per frame)" % (group["name"], group["reference"], reference_frames, record["width"], record["height"],
+			record["accumulate_ms_per_frame"]), flush=True)
+		e = record["reference_frame_error"]
+		print("  %-70s relMSE %.4e  MSE %.4e" % ("(one frame of the reference's settings)", sum(e["rel_mse"]) / 3.0, sum(e["mse"]) / 3.0), flush=True)
+		for m in sorted(record["members"], key=lambda m: sum(m["rel_mse"])):
+			print("  %-70s relMSE %.4e  MSE %.4e  mean variance %s" % (m["name"], sum(m["rel_mse"]) / 3.0, sum(m["mse"]) / 3.0,
+				"%.4e" % (sum(m["mean_variance"]) / 3.0) if m["mean_variance"] else "-"), flush=True)
+	os.makedirs(os.path.dirname(os.path.abspath(json_path)), exist_ok=True)
+	with open(json_path, "w") as f:
+		json.dump(records, f, indent=1)
 	return records
