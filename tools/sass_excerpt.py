@@ -14,7 +14,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 KERNEL = "_ZN3vkr14shading_kernelILi3ELi5ELb0ELb0ELb1EEEvNS_21shading_kernel_paramsE"
-OBJ = os.path.join(ROOT, "vulkan_renderer_b200", "build", "vkr_shading_kernel_maxp5.cu.o")
+OBJ = os.path.join(ROOT, "vulkan_renderer_b200", "build", "vkr_shading_kernel_v4.cu.o")
 
 
 def main():
@@ -27,7 +27,7 @@ def main():
 	def family(prefixes): return sum(v for k, v in ops.items() if k.split(".")[0] in prefixes)
 	git = subprocess.run(["git", "-C", ROOT, "rev-parse", "--short", "HEAD"], stdout=subprocess.PIPE, text=True).stdout.strip()
 	out = ["# SASS of `shading_kernel<3,5,0,0,1>` (sm_90a), commit %s" % git, "",
-		"`cuobjdump -sass -fun %s vulkan_renderer_b200/build/vkr_shading_kernel_maxp5.cu.o`, excerpts." % KERNEL, "",
+		"`cuobjdump -sass -fun %s vulkan_renderer_b200/build/vkr_shading_kernel_v4.cu.o`, excerpts." % KERNEL, "",
 		"* resource usage: `%s`" % (usage[0] if usage else "?"),
 		"* %d instructions; FFMA / FMUL / FADD %d, FMNMX %d, VIMNMX3 / VIMNMX %d, MUFU %d, LDG %d (of them 128-bit: %d), LDS / STS %d, LDL / STL (spills) %d, VOTE / SHFL %d" % (
 			len(lines), family({"FFMA", "FMUL", "FADD"}), family({"FMNMX"}), family({"VIMNMX3", "VIMNMX"}), family({"MUFU"}), family({"LDG"}), sum(v for k, v in ops.items() if k.startswith("LDG") and ".128" in k),

@@ -61,8 +61,8 @@ def sass_profile(rep):
 
 
 def line_info(kernel_mangled_regex, maxp):
-	"""SASS line table of the kernel from the in-tree object of its vertex bound (build/vkr_shading_kernel_maxp<k>.cu.o)."""
-	obj = os.path.join(ROOT, "vulkan_renderer_b200", "build", "vkr_shading_kernel_maxp%s.cu.o" % maxp)
+	"""SASS line table of the kernel from the in-tree object of its vertex bound (build/vkr_shading_kernel_v<maxp - 1>.cu.o)."""
+	obj = os.path.join(ROOT, "vulkan_renderer_b200", "build", "vkr_shading_kernel_v%d.cu.o" % (int(maxp) - 1))
 	if not os.path.exists(obj):
 		return []
 	tmp = tempfile.mkdtemp()

@@ -2,7 +2,7 @@
 // which keeps a variant library at a tenth of the size of the product library (they travel to the GPU box with every call).
 #include "../vulkan_renderer_b200/csrc/vkr_kernels.h"
 #define VKR_STUB(name) cudaError_t name(const vkr::shading_kernel_params&, cudaStream_t) { return cudaErrorNotSupported; }
-VKR_STUB(vkr_launch_shading_kernel_maxp4) VKR_STUB(vkr_launch_shading_kernel_maxp6) VKR_STUB(vkr_launch_shading_kernel_maxp7) VKR_STUB(vkr_launch_shading_kernel_maxp8)
-VKR_STUB(vkr_launch_textured_light_kernel_maxp4) VKR_STUB(vkr_launch_textured_light_kernel_maxp5) VKR_STUB(vkr_launch_textured_light_kernel_maxp6) VKR_STUB(vkr_launch_textured_light_kernel_maxp7) VKR_STUB(vkr_launch_textured_light_kernel_maxp8)
-VKR_STUB(vkr_launch_textured_related_work_kernel_maxv3) VKR_STUB(vkr_launch_textured_related_work_kernel_maxv4) VKR_STUB(vkr_launch_textured_related_work_kernel_maxv5) VKR_STUB(vkr_launch_textured_related_work_kernel_maxv6) VKR_STUB(vkr_launch_textured_related_work_kernel_maxv7)
-VKR_STUB(vkr_launch_related_work_kernel_maxv3) VKR_STUB(vkr_launch_related_work_kernel_maxv4) VKR_STUB(vkr_launch_related_work_kernel_maxv5) VKR_STUB(vkr_launch_related_work_kernel_maxv6) VKR_STUB(vkr_launch_related_work_kernel_maxv7)
+VKR_STUB(vkr_launch_shading_kernel_v3) VKR_STUB(vkr_launch_shading_kernel_v5) VKR_STUB(vkr_launch_shading_kernel_v6) VKR_STUB(vkr_launch_shading_kernel_v7)
+VKR_STUB(vkr_launch_textured_light_kernel_v3) VKR_STUB(vkr_launch_textured_light_kernel_v4) VKR_STUB(vkr_launch_textured_light_kernel_v5) VKR_STUB(vkr_launch_textured_light_kernel_v6) VKR_STUB(vkr_launch_textured_light_kernel_v7)
+VKR_STUB(vkr_launch_textured_related_work_kernel_v3) VKR_STUB(vkr_launch_textured_related_work_kernel_v4) VKR_STUB(vkr_launch_textured_related_work_kernel_v5) VKR_STUB(vkr_launch_textured_related_work_kernel_v6) VKR_STUB(vkr_launch_textured_related_work_kernel_v7)
+VKR_STUB(vkr_launch_related_work_kernel_v3) VKR_STUB(vkr_launch_related_work_kernel_v4) VKR_STUB(vkr_launch_related_work_kernel_v5) VKR_STUB(vkr_launch_related_work_kernel_v6) VKR_STUB(vkr_launch_related_work_kernel_v7)

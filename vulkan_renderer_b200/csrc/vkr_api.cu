@@ -186,45 +186,22 @@ static void reorder_tiles_by_cost(vkr_shading_pass_t* pass) {
 	std::stable_sort(list, list + pass->tile_count, [cost](uint32_t a, uint32_t b) { return cost[a] > cost[b]; });
 }
 
+// The tile kernels by family and by MAX_POLYGONAL_LIGHT_VERTEX_COUNT = 3 .. 7, a compile-time bound of the kernels
+enum { FAMILY_TEXTURED_RELATED_WORK, FAMILY_RELATED_WORK, FAMILY_TEXTURED_LIGHTS, FAMILY_PROJECTED_SOLID_ANGLE };
+static vkr_tile_launcher_t* const kTileLaunchers[4][5] = {
+	{vkr_launch_textured_related_work_kernel_v3, vkr_launch_textured_related_work_kernel_v4, vkr_launch_textured_related_work_kernel_v5, vkr_launch_textured_related_work_kernel_v6, vkr_launch_textured_related_work_kernel_v7},
+	{vkr_launch_related_work_kernel_v3, vkr_launch_related_work_kernel_v4, vkr_launch_related_work_kernel_v5, vkr_launch_related_work_kernel_v6, vkr_launch_related_work_kernel_v7},
+	{vkr_launch_textured_light_kernel_v3, vkr_launch_textured_light_kernel_v4, vkr_launch_textured_light_kernel_v5, vkr_launch_textured_light_kernel_v6, vkr_launch_textured_light_kernel_v7},
+	{vkr_launch_shading_kernel_v3, vkr_launch_shading_kernel_v4, vkr_launch_shading_kernel_v5, vkr_launch_shading_kernel_v6, vkr_launch_shading_kernel_v7},
+};
+
 cudaError_t vkr_launch_shading_kernel(const vkr::shading_kernel_params& p, cudaStream_t stream) {
-	if (p.light_texture_count != 0 && p.polygon_sampling_technique < 11 && p.error_display == 0) { // related-work techniques under textured lights
-		switch (p.max_light_vertex_count) {
-		case 3: return vkr_launch_textured_related_work_kernel_maxv3(p, stream);
-		case 4: return vkr_launch_textured_related_work_kernel_maxv4(p, stream);
-		case 5: return vkr_launch_textured_related_work_kernel_maxv5(p, stream);
-		case 6: return vkr_launch_textured_related_work_kernel_maxv6(p, stream);
-		case 7: return vkr_launch_textured_related_work_kernel_maxv7(p, stream);
-		default: return cudaErrorInvalidValue;
-		}
-	}
-	if (p.polygon_sampling_technique < 11 || p.error_display != 0) { // related-work techniques and error display (SURVEY 8 f4)
-		switch (p.max_light_vertex_count) {
-		case 3: return vkr_launch_related_work_kernel_maxv3(p, stream);
-		case 4: return vkr_launch_related_work_kernel_maxv4(p, stream);
-		case 5: return vkr_launch_related_work_kernel_maxv5(p, stream);
-		case 6: return vkr_launch_related_work_kernel_maxv6(p, stream);
-		case 7: return vkr_launch_related_work_kernel_maxv7(p, stream);
-		default: return cudaErrorInvalidValue;
-		}
-	}
-	if (p.light_texture_count != 0) { // at least one textured light in this frame (vkr_textured_light_kernel.cu)
-		switch (p.max_light_vertex_count) {
-		case 3: return vkr_launch_textured_light_kernel_maxp4(p, stream);
-		case 4: return vkr_launch_textured_light_kernel_maxp5(p, stream);
-		case 5: return vkr_launch_textured_light_kernel_maxp6(p, stream);
-		case 6: return vkr_launch_textured_light_kernel_maxp7(p, stream);
-		case 7: return vkr_launch_textured_light_kernel_maxp8(p, stream);
-		default: return cudaErrorInvalidValue;
-		}
-	}
-	switch (p.max_light_vertex_count) { // MAX_POLYGONAL_LIGHT_VERTEX_COUNT, a compile-time bound of the kernels
-	case 3: return vkr_launch_shading_kernel_maxp4(p, stream);
-	case 4: return vkr_launch_shading_kernel_maxp5(p, stream);
-	case 5: return vkr_launch_shading_kernel_maxp6(p, stream);
-	case 6: return vkr_launch_shading_kernel_maxp7(p, stream);
-	case 7: return vkr_launch_shading_kernel_maxp8(p, stream);
-	default: return cudaErrorInvalidValue;
-	}
+	int family = FAMILY_PROJECTED_SOLID_ANGLE;
+	if (p.light_texture_count != 0 && p.polygon_sampling_technique < 11 && p.error_display == 0) family = FAMILY_TEXTURED_RELATED_WORK; // related-work techniques under textured lights
+	else if (p.polygon_sampling_technique < 11 || p.error_display != 0) family = FAMILY_RELATED_WORK; // related-work techniques and error display (SURVEY 8 f4)
+	else if (p.light_texture_count != 0) family = FAMILY_TEXTURED_LIGHTS; // at least one textured light in this frame
+	if (p.max_light_vertex_count < 3 || p.max_light_vertex_count > 7) return cudaErrorInvalidValue;
+	return kTileLaunchers[family][p.max_light_vertex_count - 3](p, stream);
 }
 
 // exchange: when not null, the pixels also go into the frames of the other GPUs (vkr_exchange.cu fills peer_outs)
@@ -326,7 +303,7 @@ int vkr_launch_shading(vkr_shading_pass_t* pass, const vkr_device_t* device, con
 		p.stats = d_stats;
 	}
 	if (pass->timing_enabled) cudaEventRecord((cudaEvent_t) pass->event_begin, stream);
-	cudaError_t err = d_stats ? vkr_launch_shading_kernel_stats_maxp5(p, stream) : vkr_launch_shading_kernel(p, stream);
+	cudaError_t err = d_stats ? vkr_launch_shading_kernel_stats_v4(p, stream) : vkr_launch_shading_kernel(p, stream);
 	if (pass->timing_enabled) cudaEventRecord((cudaEvent_t) pass->event_end, stream);
 	VKR_CUDA_OK(err, "Failed to launch the shading kernel");
 	++pass->kernel_launches;

@@ -66,27 +66,17 @@ struct gbuffer_kernel_params {
 } // namespace vkr
 
 cudaError_t vkr_launch_shading_kernel(const vkr::shading_kernel_params& p, cudaStream_t stream);   // dispatches on max_light_vertex_count (vkr_api.cu)
-cudaError_t vkr_launch_shading_kernel_maxp4(const vkr::shading_kernel_params& p, cudaStream_t stream); // vkr_shading_kernel.cu, one object per vertex bound
-cudaError_t vkr_launch_shading_kernel_maxp5(const vkr::shading_kernel_params& p, cudaStream_t stream);
-cudaError_t vkr_launch_shading_kernel_maxp6(const vkr::shading_kernel_params& p, cudaStream_t stream);
-cudaError_t vkr_launch_shading_kernel_maxp7(const vkr::shading_kernel_params& p, cudaStream_t stream);
-cudaError_t vkr_launch_shading_kernel_maxp8(const vkr::shading_kernel_params& p, cudaStream_t stream);
-cudaError_t vkr_launch_shading_kernel_stats_maxp5(const vkr::shading_kernel_params& p, cudaStream_t stream); // the counters edition of the quad-light kernels (-DVKR_TRACE_STATS)
-cudaError_t vkr_launch_textured_light_kernel_maxp4(const vkr::shading_kernel_params& p, cudaStream_t stream); // vkr_textured_light_kernel.cu, frames with textured lights
-cudaError_t vkr_launch_textured_light_kernel_maxp5(const vkr::shading_kernel_params& p, cudaStream_t stream);
-cudaError_t vkr_launch_textured_light_kernel_maxp6(const vkr::shading_kernel_params& p, cudaStream_t stream);
-cudaError_t vkr_launch_textured_light_kernel_maxp7(const vkr::shading_kernel_params& p, cudaStream_t stream);
-cudaError_t vkr_launch_textured_light_kernel_maxp8(const vkr::shading_kernel_params& p, cudaStream_t stream);
-cudaError_t vkr_launch_textured_related_work_kernel_maxv3(const vkr::shading_kernel_params& p, cudaStream_t stream); // vkr_textured_related_work_kernel.cu
-cudaError_t vkr_launch_textured_related_work_kernel_maxv4(const vkr::shading_kernel_params& p, cudaStream_t stream);
-cudaError_t vkr_launch_textured_related_work_kernel_maxv5(const vkr::shading_kernel_params& p, cudaStream_t stream);
-cudaError_t vkr_launch_textured_related_work_kernel_maxv6(const vkr::shading_kernel_params& p, cudaStream_t stream);
-cudaError_t vkr_launch_textured_related_work_kernel_maxv7(const vkr::shading_kernel_params& p, cudaStream_t stream);
-cudaError_t vkr_launch_related_work_kernel_maxv3(const vkr::shading_kernel_params& p, cudaStream_t stream); // vkr_related_work_kernel.cu, one object per light vertex bound
-cudaError_t vkr_launch_related_work_kernel_maxv4(const vkr::shading_kernel_params& p, cudaStream_t stream);
-cudaError_t vkr_launch_related_work_kernel_maxv5(const vkr::shading_kernel_params& p, cudaStream_t stream);
-cudaError_t vkr_launch_related_work_kernel_maxv6(const vkr::shading_kernel_params& p, cudaStream_t stream);
-cudaError_t vkr_launch_related_work_kernel_maxv7(const vkr::shading_kernel_params& p, cudaStream_t stream);
+// The tile kernels' entry points: one object per kernel family and light vertex bound MAX_POLYGONAL_LIGHT_VERTEX_COUNT = 3 .. 7 (__graft_entry__.py)
+typedef cudaError_t vkr_tile_launcher_t(const vkr::shading_kernel_params& p, cudaStream_t stream);
+// vkr_shading_kernel.cu: projected solid angle sampling, and the counters edition of its quad-light kernels (-DVKR_TRACE_STATS)
+vkr_tile_launcher_t vkr_launch_shading_kernel_v3, vkr_launch_shading_kernel_v4, vkr_launch_shading_kernel_v5, vkr_launch_shading_kernel_v6, vkr_launch_shading_kernel_v7;
+vkr_tile_launcher_t vkr_launch_shading_kernel_stats_v4;
+// vkr_textured_light_kernel.cu: the same for frames with textured lights
+vkr_tile_launcher_t vkr_launch_textured_light_kernel_v3, vkr_launch_textured_light_kernel_v4, vkr_launch_textured_light_kernel_v5, vkr_launch_textured_light_kernel_v6, vkr_launch_textured_light_kernel_v7;
+// vkr_related_work_kernel.cu: the related-work sampling techniques and the error display
+vkr_tile_launcher_t vkr_launch_related_work_kernel_v3, vkr_launch_related_work_kernel_v4, vkr_launch_related_work_kernel_v5, vkr_launch_related_work_kernel_v6, vkr_launch_related_work_kernel_v7;
+// vkr_textured_related_work_kernel.cu: the related-work sampling techniques for frames with textured lights
+vkr_tile_launcher_t vkr_launch_textured_related_work_kernel_v3, vkr_launch_textured_related_work_kernel_v4, vkr_launch_textured_related_work_kernel_v5, vkr_launch_textured_related_work_kernel_v6, vkr_launch_textured_related_work_kernel_v7;
 // float node pairs -> quantised node pairs (vkr_lbvh_gpu.cu); d_nodes_q: 32 bytes per pair
 cudaError_t vkr_quantise_node_pairs(const float4* d_nodes, uint64_t pair_count, const float grid[6], uint4* d_nodes_q, cudaStream_t stream);
 // float node pairs -> interleaved node pairs (vkr_lbvh_gpu.cu); d_nodes_i: 64 bytes per pair

@@ -24,26 +24,22 @@
 // floating-point sums identical to the reference's sequential loop. Without shadow rays (TRACE = false) the kernel is
 // launched with the shading warps only.
 // Compile with -fmad=false (see vkr_device_math.cuh).
-#include "vkr_shading_tile.cuh"
+#include "vkr_tile_launch.cuh"
 #include "vkr_shade_light.cuh"
 
 // The counters edition (-DVKR_TRACE_STATS, vkr_trace_counter_t) is a kernel of its own name: the host stubs of two editions of one template
 // would be merged by the linker.
 #ifdef VKR_TRACE_STATS
 #define shading_kernel shading_kernel_counters
-#define VKR_LAUNCHER_PREFIX vkr_launch_shading_kernel_stats_maxp
+#define VKR_LAUNCHER_PREFIX vkr_launch_shading_kernel_stats_v
 #else
-#define VKR_LAUNCHER_PREFIX vkr_launch_shading_kernel_maxp
-#endif
-
-#ifndef VKR_TRACED_CTAS_PER_SM
-#define VKR_TRACED_CTAS_PER_SM 2   // CTAs per SM the register allocation of the kernels with shadow rays is made for (tuning knob, with VKR_SHADE_REGS / VKR_TRACE_REGS)
+#define VKR_LAUNCHER_PREFIX vkr_launch_shading_kernel_v
 #endif
 
 namespace vkr {
 
 template <int STRATEGY, int MAXP, bool BIASED, bool OPTIMAL, bool TRACE>
-__global__ void __launch_bounds__(TRACE ? kShadeThreads + kTraceThreads : kShadeThreads, TRACE ? VKR_TRACED_CTAS_PER_SM : 3)
+__global__ void VKR_TILE_LAUNCH_BOUNDS(TRACE)
 shading_kernel(const shading_kernel_params p) {
 	shade_tile<MAXP, OPTIMAL, TRACE>(p, psa_light_shader<STRATEGY, MAXP, BIASED, OPTIMAL, TRACE>());
 }
@@ -52,53 +48,29 @@ shading_kernel(const shading_kernel_params p) {
 
 using namespace vkr;
 
-template <int STRATEGY, int MAXP, bool BIASED, bool OPTIMAL, bool TRACE>
-static cudaError_t launch_traced(const shading_kernel_params& p, cudaStream_t stream) {
-	if (p.tile_count <= 0) return cudaSuccess;
-	const int threads = TRACE ? kShadeThreads + kTraceThreads : kShadeThreads;
-	const size_t smem = p.constants_smem_bytes + (TRACE ? sizeof(float) * stream_floats_per_warp(OPTIMAL) * kShadeWarps + sizeof(int) * (size_t) p.stack_depth * kTraceThreads : 0);
-	auto kernel = shading_kernel<STRATEGY, MAXP, BIASED, OPTIMAL, TRACE>;
-	cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
-	if (err != cudaSuccess) return err;
-	// Shared memory for exactly the CTAs the register file admits; the rest of the 228 KB stays L1 for BVH nodes
-	int ctas = 0;
-	err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, kernel, threads, smem);
-	if (err != cudaSuccess) return err;
-	const int carveout = (int) ((100 * ((smem + 1024) * (size_t) (ctas > 0 ? ctas : 1)) + 228 * 1024 - 1) / (228 * 1024));
-	err = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carveout > 100 ? 100 : carveout);
-	if (err != cudaSuccess) return err;
-	kernel<<<p.tile_count, threads, smem, stream>>>(p);
-	return cudaGetLastError();
+constexpr int kMaxP = VKR_MAXV_TU + 1;   // MAXP: vertices of a light after clipping to the horizon
+
+// the kernels of one strategy, with and without shadow rays
+template <int STRATEGY, bool BIASED, bool OPTIMAL = false>
+static cudaError_t launch(const shading_kernel_params& p, cudaStream_t stream) {
+	return launch_tile_kernel<OPTIMAL>(shading_kernel<STRATEGY, kMaxP, BIASED, OPTIMAL, true>, shading_kernel<STRATEGY, kMaxP, BIASED, OPTIMAL, false>, p, stream);
 }
 
-template <int STRATEGY, int MAXP, bool BIASED, bool OPTIMAL>
-static cudaError_t launch_variant(const shading_kernel_params& p, cudaStream_t stream) {
-	if (p.trace_shadow_rays != 0 && p.tri_count != 0) return launch_traced<STRATEGY, MAXP, BIASED, OPTIMAL, true>(p, stream);
-	return launch_traced<STRATEGY, MAXP, BIASED, OPTIMAL, false>(p, stream);
-}
-
-template <int MAXP, bool BIASED>
+template <bool BIASED>
 static cudaError_t launch_strategy(const shading_kernel_params& p, cudaStream_t stream) {
 	switch (p.sampling_strategies) {
-	case VKR_STRATEGY_DIFFUSE_ONLY: return launch_variant<VKR_STRATEGY_DIFFUSE_ONLY, MAXP, BIASED, false>(p, stream);
-	case VKR_STRATEGY_DIFFUSE_GGX_MIS: return launch_variant<VKR_STRATEGY_DIFFUSE_GGX_MIS, MAXP, BIASED, false>(p, stream);
-	case VKR_STRATEGY_DIFFUSE_SPECULAR_SEPARATELY: return launch_variant<VKR_STRATEGY_DIFFUSE_SPECULAR_SEPARATELY, MAXP, BIASED, false>(p, stream);
+	case VKR_STRATEGY_DIFFUSE_ONLY: return launch<VKR_STRATEGY_DIFFUSE_ONLY, BIASED>(p, stream);
+	case VKR_STRATEGY_DIFFUSE_GGX_MIS: return launch<VKR_STRATEGY_DIFFUSE_GGX_MIS, BIASED>(p, stream);
+	case VKR_STRATEGY_DIFFUSE_SPECULAR_SEPARATELY: return launch<VKR_STRATEGY_DIFFUSE_SPECULAR_SEPARATELY, BIASED>(p, stream);
 	case VKR_STRATEGY_DIFFUSE_SPECULAR_MIS:
-		if (p.mis_heuristic == VKR_MIS_OPTIMAL) return launch_variant<VKR_STRATEGY_DIFFUSE_SPECULAR_MIS, MAXP, BIASED, true>(p, stream);
-		return launch_variant<VKR_STRATEGY_DIFFUSE_SPECULAR_MIS, MAXP, BIASED, false>(p, stream);
-	case VKR_STRATEGY_DIFFUSE_SPECULAR_RANDOM: return launch_variant<VKR_STRATEGY_DIFFUSE_SPECULAR_RANDOM, MAXP, BIASED, false>(p, stream);
+		if (p.mis_heuristic == VKR_MIS_OPTIMAL) return launch<VKR_STRATEGY_DIFFUSE_SPECULAR_MIS, BIASED, true>(p, stream);
+		return launch<VKR_STRATEGY_DIFFUSE_SPECULAR_MIS, BIASED>(p, stream);
+	case VKR_STRATEGY_DIFFUSE_SPECULAR_RANDOM: return launch<VKR_STRATEGY_DIFFUSE_SPECULAR_RANDOM, BIASED>(p, stream);
 	default: return cudaErrorInvalidValue;
 	}
 }
 
-// One translation unit per vertex bound (built with -DVKR_MAXP_TU=4 .. 8, __graft_entry__.py): MAXP = light vertices + 1.
-#ifndef VKR_MAXP_TU
-#error "compile with -DVKR_MAXP_TU=<4..8>"
-#endif
-#define VKR_CONCAT2(a, b) a##b
-#define VKR_CONCAT(a, b) VKR_CONCAT2(a, b)
-cudaError_t VKR_CONCAT(VKR_LAUNCHER_PREFIX, VKR_MAXP_TU)(const shading_kernel_params& p, cudaStream_t stream) {
-	if (p.stack_depth < 2 || p.stack_depth > kMaxStackDepth) return cudaErrorInvalidValue;
-	if (p.trace_shadow_rays != 0 && p.tri_count != 0 && p.bvh_width != VKR_BVH_WIDTH) return cudaErrorInvalidValue; // the scene's BVH layout must be the one these kernels walk
-	return p.biased_sampling ? launch_strategy<VKR_MAXP_TU, true>(p, stream) : launch_strategy<VKR_MAXP_TU, false>(p, stream);
+cudaError_t VKR_TILE_LAUNCHER(VKR_LAUNCHER_PREFIX)(const shading_kernel_params& p, cudaStream_t stream) {
+	if (!tile_launch_valid(p, false)) return cudaErrorInvalidValue;
+	return p.biased_sampling ? launch_strategy<true>(p, stream) : launch_strategy<false>(p, stream);
 }

@@ -21,6 +21,9 @@ constexpr int kTraceThreads = 32 * kTraceWarps;
 #ifndef VKR_TRACE_REGS
 #define VKR_TRACE_REGS 56
 #endif
+// Dynamic shared memory of a tile: the constant block (constants_smem_bytes), then, with shadow rays, the ray streams of the shading warps (these
+// bytes) and the traversal stacks of the trace lanes (stack_depth ints each). tile_smem_bytes() (vkr_tile_launch.cuh) sizes launches by it.
+VKR_DEV constexpr size_t tile_streams_bytes(bool optimal) { return sizeof(float) * stream_floats_per_warp(optimal) * kShadeWarps; }
 
 // LightShader: void operator()(bool on, const shading_point&, const ltc_state&, const unsigned char* light, noise_stream&,
 //   const shading_kernel_params&, const unsigned char* cb, uint32_t px, uint32_t py, ray_producer&, pixel_sum&, int lane) const
@@ -31,7 +34,7 @@ VKR_DEV void shade_tile(const shading_kernel_params& p, const LightShader& shade
 	extern __shared__ __align__(16) unsigned char smem[];
 	unsigned char* cb = smem;                                   // constant block incl. lights
 	float* stream_base = reinterpret_cast<float*>(smem + p.constants_smem_bytes);
-	int* stack_base = reinterpret_cast<int*>(stream_base + stream_floats_per_warp(OPTIMAL) * kShadeWarps);
+	int* stack_base = reinterpret_cast<int*>(smem + p.constants_smem_bytes + tile_streams_bytes(OPTIMAL));
 	__shared__ __align__(8) unsigned long long mbar;
 	const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 	// --- stage the constant block with one bulk async copy (TMA engine), completion on an mbarrier

@@ -9,7 +9,7 @@
 // and in the light display of the tile prologue. vkr_api.cu sends a frame here when at least one light of the constant block is textured.
 // The biased variant of the sampler is a run-time choice inside the kernel (half as many kernels to compile; the choice is uniform).
 // Compile with -fmad=false (see vkr_device_math.cuh).
-#include "vkr_shading_tile.cuh"
+#include "vkr_tile_launch.cuh"
 #include "vkr_shade_light.cuh"
 
 namespace vkr {
@@ -25,7 +25,7 @@ struct textured_light_shader {
 };
 
 template <int STRATEGY, int MAXP, bool OPTIMAL, bool TRACE>
-__global__ void __launch_bounds__(TRACE ? kShadeThreads + kTraceThreads : kShadeThreads, TRACE ? 2 : 3)
+__global__ void VKR_TILE_LAUNCH_BOUNDS(TRACE)
 textured_light_kernel(const shading_kernel_params p) {
 	shade_tile<MAXP, OPTIMAL, TRACE, true>(p, textured_light_shader<STRATEGY, MAXP, OPTIMAL, TRACE>());
 }
@@ -34,49 +34,24 @@ textured_light_kernel(const shading_kernel_params p) {
 
 using namespace vkr;
 
-template <int STRATEGY, int MAXP, bool OPTIMAL, bool TRACE>
-static cudaError_t launch_traced(const shading_kernel_params& p, cudaStream_t stream) {
-	if (p.tile_count <= 0) return cudaSuccess;
-	const int threads = TRACE ? kShadeThreads + kTraceThreads : kShadeThreads;
-	constexpr size_t stream_floats = stream_floats_per_warp(OPTIMAL);
-	const size_t smem = p.constants_smem_bytes + (TRACE ? sizeof(float) * stream_floats * kShadeWarps + sizeof(int) * (size_t) p.stack_depth * kTraceThreads : 0);
-	auto kernel = textured_light_kernel<STRATEGY, MAXP, OPTIMAL, TRACE>;
-	cudaError_t err = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem);
-	if (err != cudaSuccess) return err;
-	int ctas = 0;
-	err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ctas, kernel, threads, smem);
-	if (err != cudaSuccess) return err;
-	const int carveout = (int) ((100 * ((smem + 1024) * (size_t) (ctas > 0 ? ctas : 1)) + 228 * 1024 - 1) / (228 * 1024));
-	err = cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, carveout > 100 ? 100 : carveout);
-	if (err != cudaSuccess) return err;
-	kernel<<<p.tile_count, threads, smem, stream>>>(p);
-	return cudaGetLastError();
+constexpr int kMaxP = VKR_MAXV_TU + 1;   // MAXP: vertices of a light after clipping to the horizon
+
+// the kernels of one strategy, with and without shadow rays
+template <int STRATEGY, bool OPTIMAL = false>
+static cudaError_t launch(const shading_kernel_params& p, cudaStream_t stream) {
+	return launch_tile_kernel<OPTIMAL>(textured_light_kernel<STRATEGY, kMaxP, OPTIMAL, true>, textured_light_kernel<STRATEGY, kMaxP, OPTIMAL, false>, p, stream);
 }
 
-template <int STRATEGY, int MAXP, bool OPTIMAL>
-static cudaError_t launch_variant(const shading_kernel_params& p, cudaStream_t stream) {
-	if (p.trace_shadow_rays != 0 && p.tri_count != 0) return launch_traced<STRATEGY, MAXP, OPTIMAL, true>(p, stream);
-	return launch_traced<STRATEGY, MAXP, OPTIMAL, false>(p, stream);
-}
-
-// One translation unit per vertex bound (built with -DVKR_MAXP_TU=4 .. 8, __graft_entry__.py): MAXP = light vertices + 1.
-#ifndef VKR_MAXP_TU
-#error "compile with -DVKR_MAXP_TU=<4..8>"
-#endif
-#define VKR_CONCAT2(a, b) a##b
-#define VKR_CONCAT(a, b) VKR_CONCAT2(a, b)
-cudaError_t VKR_CONCAT(vkr_launch_textured_light_kernel_maxp, VKR_MAXP_TU)(const shading_kernel_params& p, cudaStream_t stream) {
-	if (p.stack_depth < 2 || p.stack_depth > kMaxStackDepth) return cudaErrorInvalidValue;
-	if (p.trace_shadow_rays != 0 && p.tri_count != 0 && p.bvh_width != VKR_BVH_WIDTH) return cudaErrorInvalidValue;
-	if (!p.light_texture_texels || !p.light_texture_dims || !p.light_texture_offsets || p.light_texture_count == 0) return cudaErrorInvalidValue;
+cudaError_t VKR_TILE_LAUNCHER(vkr_launch_textured_light_kernel_v)(const shading_kernel_params& p, cudaStream_t stream) {
+	if (!tile_launch_valid(p, true)) return cudaErrorInvalidValue;
 	switch (p.sampling_strategies) {
-	case VKR_STRATEGY_DIFFUSE_ONLY: return launch_variant<VKR_STRATEGY_DIFFUSE_ONLY, VKR_MAXP_TU, false>(p, stream);
-	case VKR_STRATEGY_DIFFUSE_GGX_MIS: return launch_variant<VKR_STRATEGY_DIFFUSE_GGX_MIS, VKR_MAXP_TU, false>(p, stream);
-	case VKR_STRATEGY_DIFFUSE_SPECULAR_SEPARATELY: return launch_variant<VKR_STRATEGY_DIFFUSE_SPECULAR_SEPARATELY, VKR_MAXP_TU, false>(p, stream);
+	case VKR_STRATEGY_DIFFUSE_ONLY: return launch<VKR_STRATEGY_DIFFUSE_ONLY>(p, stream);
+	case VKR_STRATEGY_DIFFUSE_GGX_MIS: return launch<VKR_STRATEGY_DIFFUSE_GGX_MIS>(p, stream);
+	case VKR_STRATEGY_DIFFUSE_SPECULAR_SEPARATELY: return launch<VKR_STRATEGY_DIFFUSE_SPECULAR_SEPARATELY>(p, stream);
 	case VKR_STRATEGY_DIFFUSE_SPECULAR_MIS:
-		if (p.mis_heuristic == VKR_MIS_OPTIMAL) return launch_variant<VKR_STRATEGY_DIFFUSE_SPECULAR_MIS, VKR_MAXP_TU, true>(p, stream);
-		return launch_variant<VKR_STRATEGY_DIFFUSE_SPECULAR_MIS, VKR_MAXP_TU, false>(p, stream);
-	case VKR_STRATEGY_DIFFUSE_SPECULAR_RANDOM: return launch_variant<VKR_STRATEGY_DIFFUSE_SPECULAR_RANDOM, VKR_MAXP_TU, false>(p, stream);
+		if (p.mis_heuristic == VKR_MIS_OPTIMAL) return launch<VKR_STRATEGY_DIFFUSE_SPECULAR_MIS, true>(p, stream);
+		return launch<VKR_STRATEGY_DIFFUSE_SPECULAR_MIS>(p, stream);
+	case VKR_STRATEGY_DIFFUSE_SPECULAR_RANDOM: return launch<VKR_STRATEGY_DIFFUSE_SPECULAR_RANDOM>(p, stream);
 	default: return cudaErrorInvalidValue;
 	}
 }

@@ -551,6 +551,9 @@ def build_dataset(directory, name, **overrides):
 		for i, light in enumerate(lights):
 			light["texturing_technique"] = 1 + i % 3
 			light["texture_file_path"] = paths[i % 3]
+			if overrides.get("vertices"):   # regular polygons of 3 .. 7 vertices instead of quads, as in mini_v5
+				n = int(overrides["vertices"]); phase = 0.3 * n
+				light["vertices"] = [(0.5 + 0.5 * float(np.cos(phase + 2.0 * np.pi * k / n)), 0.5 + 0.5 * float(np.sin(phase + 2.0 * np.pi * k / n))) for k in range(n)]
 	elif name in ("mini_tri", "mini_mixed"):
 		# the mini_city scene lit by triangles (MAX_POLYGONAL_LIGHT_VERTEX_COUNT = 3) or by a triangle, a quad and a
 		# triangle (MIN_POLYGON_VERTEX_COUNT_BEFORE_CLIPPING = 3 < MAX = 4, main.c:730-732)
