@@ -178,6 +178,37 @@ int vkr_ltc_table_from_images(vkr_ltc_table_t* table, const vkr_device_t* device
 	const uint16_t* table0_rgba16, const uint16_t* table1_rg16, const vkr_ltc_constants_t* constants);
 void vkr_destroy_ltc_table(vkr_ltc_table_t* table, const vkr_device_t* device);
 
+/* ---- fitting the LTC table (no counterpart in the reference, which reads fit<i>.dat from its data download): the specular BRDF of
+        brdfs.glsl:74-87 (GGX, height-correlated Smith, Fresnel-Schlick with scalar F0) times cos(theta_i), fitted cell by cell with Heitz et al.
+        2016's L3 error on the device, in float64 and a fixed summation order (csrc/vkr_ltc_fit.cuh, DESIGN.md §5): bit-identical from call to call
+        and from device to device. Cell (layer f, row i, column j): F0 = f / (F - 1), theta = i / (N - 1) * pi / 2 (at most 89.5 degrees),
+        alpha = (j / (N - 1))^2 (at least 1e-3) -- the cells vkr_load_ltc_table's texture coordinates address. Files are the interchange:
+        vkr_write_ltc_fits, then vkr_load_ltc_table. */
+#define VKR_LTC_FIT_MAX_RESOLUTION 4096      /* the loader's limit */
+#define VKR_LTC_FIT_MAX_FRESNEL_COUNT 1024
+#define VKR_LTC_FIT_MAX_QUADRATURE_SIZE 256
+#define VKR_LTC_FIT_MAX_ITERATION_LIMIT 100000
+typedef struct vkr_ltc_fit_desc_s {
+	uint32_t resolution;        /* N: roughness and inclination count, 2 .. VKR_LTC_FIT_MAX_RESOLUTION (default 64) */
+	uint32_t fresnel_count;     /* F: layers, one fit<i>.dat each, 2 .. VKR_LTC_FIT_MAX_FRESNEL_COUNT (default 51) */
+	uint32_t quadrature_size;   /* n: each objective evaluation takes n x n stratified samples of the BRDF and of the LTC, 2 .. 256 (default 32) */
+	uint32_t iteration_limit;   /* Nelder-Mead iterations per cell, 1 .. VKR_LTC_FIT_MAX_ITERATION_LIMIT (default 400) */
+} vkr_ltc_fit_desc_t;
+typedef struct vkr_ltc_fit_stats_s {
+	uint64_t cell_count;
+	uint64_t objective_evaluations;   /* summed over the cells */
+	uint64_t iteration_limit_hits;    /* cells whose minimiser stopped at the iteration limit */
+	double max_error, median_error, mean_error;   /* the final L3 error of the cells (integral of |lobe / albedo - LTC|^3 over the sphere) */
+	float fit_ms;                     /* device time of the fit kernel (CUDA events) */
+	double* cell_errors;              /* set by the caller: NULL, or F * N * N doubles that receive the final L3 error per cell, [F][N][N] */
+} vkr_ltc_fit_stats_t;
+void vkr_ltc_fit_default_desc(vkr_ltc_fit_desc_t* desc);
+/* Synchronous. out_fits: HOST array [F][N][N][5] of {m00, m02, m11, m20, albedo}, texel row * N + column as in the file. stats may be NULL. */
+int vkr_fit_ltc_table(const vkr_device_t* device, const vkr_ltc_fit_desc_t* desc, float* out_fits, vkr_ltc_fit_stats_t* stats);
+/* Writes directory/fit<i>.dat, i < fresnel_count, as src/ltc_table.c:46-84 reads them: uint64 resolution, then N * N records of 5 float32.
+   The directory must exist. */
+int vkr_write_ltc_fits(const char* directory, uint32_t resolution, uint32_t fresnel_count, const float* fits);
+
 /* ---- noise table (replaces load_noise_table / set_noise_constants, src/noise_table.h:81-89, noise_table.c:46-168) */
 typedef struct vkr_noise_table_s {
 	uint32_t width, height, layers;

@@ -28,6 +28,7 @@ EXPORTED_SYMBOLS = [
 	"vkr_load_texture", "vkr_destroy_texture", "vkr_texture_from_levels", "vkr_scene_from_buffers", "vkr_ltc_table_from_images", "vkr_noise_table_from_image", "vkr_create_and_assign_light_textures", "vkr_destroy_light_textures",
 	"vkr_create_render_targets", "vkr_destroy_render_targets", "vkr_download_frame", "vkr_download_gbuffer", "vkr_upload_gbuffer",
 	"vkr_create_accumulator", "vkr_destroy_accumulator", "vkr_accumulator_reset", "vkr_accumulate_frame", "vkr_accumulator_resolve", "vkr_accumulator_mean_variance", "vkr_compare_frames",
+	"vkr_ltc_fit_default_desc", "vkr_fit_ltc_table", "vkr_write_ltc_fits",
 ]
 
 # enums (values = the reference's)
@@ -149,6 +150,17 @@ class FrameError(C.Structure):
 		("pixel_count", C.c_uint64), ("nonfinite_pixels", C.c_uint64)]
 
 
+class LtcFitDesc(C.Structure):
+	"""vkr_ltc_fit_desc_t: the size of an LTC table to fit and the fit's quadrature and iteration limit (include/vkr_b200.h)."""
+	_fields_ = [("resolution", C.c_uint32), ("fresnel_count", C.c_uint32), ("quadrature_size", C.c_uint32), ("iteration_limit", C.c_uint32)]
+
+
+class LtcFitStats(C.Structure):
+	"""vkr_ltc_fit_stats_t: what a fit cost and how well its cells fit; cell_errors is set by the caller (NULL or F * N * N doubles)."""
+	_fields_ = [("cell_count", C.c_uint64), ("objective_evaluations", C.c_uint64), ("iteration_limit_hits", C.c_uint64),
+		("max_error", C.c_double), ("median_error", C.c_double), ("mean_error", C.c_double), ("fit_ms", C.c_float), ("cell_errors", C.POINTER(C.c_double))]
+
+
 TRACE_COUNTER_NAMES = ["rays", "occluded", "cache_hits", "node_visits", "leaf_visits", "triangle_tests", "warp_rounds", "warp_node_steps", "known_occluded", "idle_polls",
 	"entries", "resolve_polls", "candidates"]   # vkr_trace_counter_t
 TRACE_COUNTER_COUNT = 16
@@ -242,5 +254,8 @@ def load_library():
 	lib.vkr_accumulator_resolve.argtypes = [P(Accumulator), P(Device), C.c_void_p, C.c_void_p]
 	lib.vkr_accumulator_mean_variance.argtypes = [P(Accumulator), P(Device), P(C.c_double)]
 	lib.vkr_compare_frames.argtypes = [P(Device), C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, P(FrameError)]
+	lib.vkr_ltc_fit_default_desc.argtypes = [P(LtcFitDesc)]; lib.vkr_ltc_fit_default_desc.restype = None
+	lib.vkr_fit_ltc_table.argtypes = [P(Device), P(LtcFitDesc), C.c_void_p, P(LtcFitStats)]
+	lib.vkr_write_ltc_fits.argtypes = [C.c_char_p, C.c_uint32, C.c_uint32, C.c_void_p]
 	_lib = lib
 	return lib

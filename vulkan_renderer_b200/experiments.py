@@ -147,10 +147,14 @@ def experiment_list(all_figs=True, all_timings=True):
 	return (figures if all_figs else []) + (timing_experiments() if all_timings else [])
 
 
-def prepare_data(experiment, data_root):
-	"""Writes the synthetic scene + quicksave an experiment names (once) and returns the dataset description."""
+def prepare_data(experiment, data_root, ltc_dir=None):
+	"""Writes the synthetic scene + quicksave an experiment names (once) and returns the dataset description. ltc_dir: a directory of fit<i>.dat
+	files (e.g. from tools/fit_ltc.py) that replaces the dataset's synthetic LTC table; None keeps it."""
 	tag = experiment["scene"] + "".join("_%s%s" % kv for kv in sorted(experiment["scene_parameters"].items()))
-	return synth.build_dataset(os.path.join(data_root, tag), experiment["scene"], **experiment["scene_parameters"])
+	info = synth.build_dataset(os.path.join(data_root, tag), experiment["scene"], **experiment["scene_parameters"])
+	if ltc_dir is not None:
+		info = dict(info, ltc=ltc_dir)
+	return info
 
 
 def _configure(frame, experiment):
@@ -164,11 +168,12 @@ def _configure(frame, experiment):
 		frame.configure(light_count=experiment["light_count"])
 
 
-def run_experiment(experiment, data_root, out_dir=None, frames=12, warmup=3, width=None, height=None, cuda_device=0, screenshot=True):
+def run_experiment(experiment, data_root, out_dir=None, frames=12, warmup=3, width=None, height=None, cuda_device=0, screenshot=True, ltc_dir=None):
 	"""Runs one experiment like the application does: set up scene, lights and settings, render `warmup` + `frames` frames, take the
-	median frame time, store the screenshot under its path with the time in milliseconds filled in. Returns the JSON record."""
+	median frame time, store the screenshot under its path with the time in milliseconds filled in. Returns the JSON record.
+	ltc_dir: LTC table to shade with instead of the synthetic one (prepare_data)."""
 	from .frame import Frame
-	info = prepare_data(experiment, data_root)
+	info = prepare_data(experiment, data_root, ltc_dir)
 	width = width or experiment["width"]; height = height or experiment["height"]
 	frame = Frame(info["vks"], info["textures"], info["save"], info["ltc"], cuda_device=cuda_device)
 	lib = frame.lib
@@ -244,18 +249,18 @@ def convergence_groups():
 	]
 
 
-def run_convergence(group, data_root, out_dir, reference_frames, variance_frames, width=None, height=None, cuda_device=0):
+def run_convergence(group, data_root, out_dir, reference_frames, variance_frames, width=None, height=None, cuda_device=0, ltc_dir=None):
 	"""Measures the members of one convergence group (convergence_groups()) against a converged reference: the reference experiment's settings
 	averaged over `reference_frames` animated frames. Per member: its screenshot frame (animate_noise = 0, the frame run_experiment shades, in linear
 	radiance) against that reference, and the mean per-frame variance over `variance_frames` animated frames. The record also holds the error of the
 	reference experiment's own screenshot frame (reference_frame_error). With out_dir, the reference is stored as out_dir/convergence/<group>_reference.hdr.
-	Returns the JSON record."""
+	ltc_dir: LTC table for the reference and the members instead of the synthetic one (prepare_data). Returns the JSON record."""
 	from . import convergence
 	from .frame import Frame
 	by_name = {e["name"]: e for e in experiment_list(all_timings=False)}
 
 	def open_frame(experiment):
-		info = prepare_data(experiment, data_root)
+		info = prepare_data(experiment, data_root, ltc_dir)
 		frame = Frame(info["vks"], info["textures"], info["save"], info["ltc"], cuda_device=cuda_device)
 		_configure(frame, experiment)
 		return frame
@@ -274,7 +279,7 @@ def run_convergence(group, data_root, out_dir, reference_frames, variance_frames
 			frame._check(frame.lib.vkr_write_hdr(path.encode(), w, h, rgb.ctypes.data), "vkr_write_hdr")
 	finally:
 		frame.close()
-	record = dict(group=group["name"], reference=group["reference"], width=w, height=h, reference_frames=reference_frames,
+	record = dict(group=group["name"], reference=group["reference"], width=w, height=h, ltc=ltc_dir or "synthetic", reference_frames=reference_frames,
 		reference_samples_per_pixel=ref_experiment["settings"]["sample_count"] * reference_frames,
 		reference_mean_variance=list(reference.mean_variance) if reference.mean_variance is not None else None,
 		reference_frame_error=reference_frame_error, accumulate_ms_per_frame=round(reference.accumulate_ms_per_frame, 5), variance_frames=variance_frames,
