@@ -223,6 +223,33 @@ int vkr_noise_table_from_image(vkr_noise_table_t* noise, const vkr_device_t* dev
 void vkr_destroy_noise_table(vkr_noise_table_t* noise, const vkr_device_t* device);
 void vkr_set_noise_constants(uint32_t resolution_mask[2], uint32_t* texture_index_mask, uint32_t random_numbers[4], vkr_noise_table_t* noise, int animate_noise);
 
+/* ---- generating the file-backed noise tables (no counterpart in the reference, which reads data/noise/<name>.blob from its data download): tables of
+        the kind vkr_noise_type_blue and vkr_noise_type_ahmed name, made on the device in integer arithmetic (csrc/vkr_noise_gen.cuh, DESIGN.md §5),
+        bit-identical from call to call and from device to device. They are this project's tables, not the paper's files. Files are the
+        interchange: vkr_write_noise_table, then vkr_load_noise_table.
+        ahmed: W = H = 2^m <= 256; each (layer, RG / BA pair) is an Owen-scrambled 2D Sobol sequence in a hierarchical pixel order, so every aligned
+               2^j x 2^j block holds a (0, 2j, 2)-net.
+        blue:  W * H <= VKR_NOISE_GEN_MAX_BLUE_PIXELS; each channel of each layer is an independent void-and-cluster dither array. */
+#define VKR_NOISE_GEN_MAX_AHMED_SIZE 256
+#define VKR_NOISE_GEN_MAX_BLUE_PIXELS 16384
+typedef struct vkr_noise_gen_desc_s {
+	vkr_noise_type_t type;          /* vkr_noise_type_blue or vkr_noise_type_ahmed */
+	uint32_t width, height, layers; /* powers of two the loader accepts (at most 9999) */
+	uint32_t seed;                  /* different seeds give independent tables */
+} vkr_noise_gen_desc_t;
+typedef struct vkr_noise_gen_stats_s {
+	float kernel_ms;                /* device time of the generating kernel (CUDA events) */
+	uint32_t relaxation_limit_hits; /* blue: dither arrays whose initial pattern stopped relaxing at the iteration limit (W * H iterations) */
+} vkr_noise_gen_stats_t;
+/* the reference's default resolution of a type (get_default_noise_resolution, src/noise_table.c:22-40): blue 64 x 64 x 64, otherwise 256 x 256 x 64 */
+void vkr_noise_gen_default_desc(vkr_noise_type_t type, vkr_noise_gen_desc_t* desc);
+/* Synchronous. texels_rgba16: HOST array of width * height * layers * 4 uint16, [layer][y][x][4] as the file holds it. stats may be NULL.
+   Refuses, before any device work: the white type, sizes the loader refuses, non-square or larger Ahmed tables, larger dither arrays, no device. */
+int vkr_generate_noise_table(const vkr_device_t* device, const vkr_noise_gen_desc_t* desc, uint16_t* texels_rgba16, vkr_noise_gen_stats_t* stats);
+/* Writes root/data/noise/blue_noise_rgba_WWxHH_LL.blob or ahmed_2d_rgba_WWxHH_LL.blob, the path vkr_load_noise_table opens relative to the working
+   directory, creating root, root/data and root/data/noise as needed (root's parent must exist). */
+int vkr_write_noise_table(const char* root, vkr_noise_type_t type, uint32_t width, uint32_t height, uint32_t layers, const uint16_t* texels_rgba16);
+
 /* ---- camera and lights (host-only; same binary layout as src/camera.h:24-44, src/polygonal_light.h:100-129) */
 typedef struct vkr_first_person_camera_s {
 	float position_world_space[3];

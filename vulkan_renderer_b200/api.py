@@ -29,6 +29,7 @@ EXPORTED_SYMBOLS = [
 	"vkr_create_render_targets", "vkr_destroy_render_targets", "vkr_download_frame", "vkr_download_gbuffer", "vkr_upload_gbuffer",
 	"vkr_create_accumulator", "vkr_destroy_accumulator", "vkr_accumulator_reset", "vkr_accumulate_frame", "vkr_accumulator_resolve", "vkr_accumulator_mean_variance", "vkr_compare_frames",
 	"vkr_ltc_fit_default_desc", "vkr_fit_ltc_table", "vkr_write_ltc_fits",
+	"vkr_noise_gen_default_desc", "vkr_generate_noise_table", "vkr_write_noise_table",
 ]
 
 # enums (values = the reference's)
@@ -161,6 +162,16 @@ class LtcFitStats(C.Structure):
 		("max_error", C.c_double), ("median_error", C.c_double), ("mean_error", C.c_double), ("fit_ms", C.c_float), ("cell_errors", C.POINTER(C.c_double))]
 
 
+class NoiseGenDesc(C.Structure):
+	"""vkr_noise_gen_desc_t: the type, size and seed of a noise table to generate (include/vkr_b200.h)."""
+	_fields_ = [("type", C.c_int), ("width", C.c_uint32), ("height", C.c_uint32), ("layers", C.c_uint32), ("seed", C.c_uint32)]
+
+
+class NoiseGenStats(C.Structure):
+	"""vkr_noise_gen_stats_t: the generating kernel's time and, for dither arrays, the relaxations stopped at the iteration limit."""
+	_fields_ = [("kernel_ms", C.c_float), ("relaxation_limit_hits", C.c_uint32)]
+
+
 TRACE_COUNTER_NAMES = ["rays", "occluded", "cache_hits", "node_visits", "leaf_visits", "triangle_tests", "warp_rounds", "warp_node_steps", "known_occluded", "idle_polls",
 	"entries", "resolve_polls", "candidates"]   # vkr_trace_counter_t
 TRACE_COUNTER_COUNT = 16
@@ -257,5 +268,9 @@ def load_library():
 	lib.vkr_ltc_fit_default_desc.argtypes = [P(LtcFitDesc)]; lib.vkr_ltc_fit_default_desc.restype = None
 	lib.vkr_fit_ltc_table.argtypes = [P(Device), P(LtcFitDesc), C.c_void_p, P(LtcFitStats)]
 	lib.vkr_write_ltc_fits.argtypes = [C.c_char_p, C.c_uint32, C.c_uint32, C.c_void_p]
+	lib.vkr_noise_table_from_image.argtypes = [P(NoiseTable), P(Device), C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32]
+	lib.vkr_noise_gen_default_desc.argtypes = [C.c_int, P(NoiseGenDesc)]; lib.vkr_noise_gen_default_desc.restype = None
+	lib.vkr_generate_noise_table.argtypes = [P(Device), P(NoiseGenDesc), C.c_void_p, P(NoiseGenStats)]
+	lib.vkr_write_noise_table.argtypes = [C.c_char_p, C.c_int, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p]
 	_lib = lib
 	return lib

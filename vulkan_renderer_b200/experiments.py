@@ -147,14 +147,26 @@ def experiment_list(all_figs=True, all_timings=True):
 	return (figures if all_figs else []) + (timing_experiments() if all_timings else [])
 
 
-def prepare_data(experiment, data_root, ltc_dir=None):
+def prepare_data(experiment, data_root, ltc_dir=None, noise_root=None):
 	"""Writes the synthetic scene + quicksave an experiment names (once) and returns the dataset description. ltc_dir: a directory of fit<i>.dat
-	files (e.g. from tools/fit_ltc.py) that replaces the dataset's synthetic LTC table; None keeps it."""
+	files (e.g. from tools/fit_ltc.py) that replaces the dataset's synthetic LTC table; None keeps it. noise_root: a directory holding
+	data/noise/ahmed_2d_rgba_256x256_64.blob (e.g. from tools/make_noise_tables.py) to shade with the Ahmed-Wonka table the reference's experiment
+	list names (src/experiment_list.c) instead of white noise; None keeps white noise."""
 	tag = experiment["scene"] + "".join("_%s%s" % kv for kv in sorted(experiment["scene_parameters"].items()))
 	info = synth.build_dataset(os.path.join(data_root, tag), experiment["scene"], **experiment["scene_parameters"])
 	if ltc_dir is not None:
 		info = dict(info, ltc=ltc_dir)
+	if noise_root is not None:
+		info = dict(info, noise_root=noise_root)
 	return info
+
+
+def open_dataset_frame(info, cuda_device=0):
+	"""A Frame over a dataset of prepare_data, with the noise table it names."""
+	from .frame import Frame
+	noise_root = info.get("noise_root")
+	return Frame(info["vks"], info["textures"], info["save"], info["ltc"], cuda_device=cuda_device,
+		noise_type=api.NOISE_AHMED if noise_root is not None else api.NOISE_WHITE, noise_root=noise_root)
 
 
 def _configure(frame, experiment):
@@ -168,14 +180,13 @@ def _configure(frame, experiment):
 		frame.configure(light_count=experiment["light_count"])
 
 
-def run_experiment(experiment, data_root, out_dir=None, frames=12, warmup=3, width=None, height=None, cuda_device=0, screenshot=True, ltc_dir=None):
+def run_experiment(experiment, data_root, out_dir=None, frames=12, warmup=3, width=None, height=None, cuda_device=0, screenshot=True, ltc_dir=None, noise_root=None):
 	"""Runs one experiment like the application does: set up scene, lights and settings, render `warmup` + `frames` frames, take the
 	median frame time, store the screenshot under its path with the time in milliseconds filled in. Returns the JSON record.
-	ltc_dir: LTC table to shade with instead of the synthetic one (prepare_data)."""
-	from .frame import Frame
-	info = prepare_data(experiment, data_root, ltc_dir)
+	ltc_dir: LTC table to shade with instead of the synthetic one; noise_root: Ahmed-Wonka table instead of white noise (prepare_data)."""
+	info = prepare_data(experiment, data_root, ltc_dir, noise_root)
 	width = width or experiment["width"]; height = height or experiment["height"]
-	frame = Frame(info["vks"], info["textures"], info["save"], info["ltc"], cuda_device=cuda_device)
+	frame = open_dataset_frame(info, cuda_device)
 	lib = frame.lib
 	lib.vkr_get_frame_time.restype = C.c_float
 	lib.vkr_record_frame_time.argtypes = [C.c_double]
@@ -204,6 +215,8 @@ def run_experiment(experiment, data_root, out_dir=None, frames=12, warmup=3, wid
 			frame_time_ms=round(frame_time_ms, 4), frames=frames, kernel_ms_min=round(min(kernel_ms), 4), kernel_ms_max=round(max(kernel_ms), 4),
 			msamples_per_s=round(width * height * s["sample_count"] / frame_time_ms / 1.0e3, 3) if frame_time_ms > 0 else None,
 			timed="shading kernel, CUDA events (the reference's number is the whole frame, src/main.c:2006)")
+		if noise_root is not None:
+			record["noise_root"] = noise_root
 		if screenshot and out_dir is not None:
 			path = os.path.join(out_dir, experiment["screenshot_path"] % frame_time_ms)
 			os.makedirs(os.path.dirname(path), exist_ok=True)
@@ -249,19 +262,18 @@ def convergence_groups():
 	]
 
 
-def run_convergence(group, data_root, out_dir, reference_frames, variance_frames, width=None, height=None, cuda_device=0, ltc_dir=None):
+def run_convergence(group, data_root, out_dir, reference_frames, variance_frames, width=None, height=None, cuda_device=0, ltc_dir=None, noise_root=None):
 	"""Measures the members of one convergence group (convergence_groups()) against a converged reference: the reference experiment's settings
 	averaged over `reference_frames` animated frames. Per member: its screenshot frame (animate_noise = 0, the frame run_experiment shades, in linear
 	radiance) against that reference, and the mean per-frame variance over `variance_frames` animated frames. The record also holds the error of the
 	reference experiment's own screenshot frame (reference_frame_error). With out_dir, the reference is stored as out_dir/convergence/<group>_reference.hdr.
-	ltc_dir: LTC table for the reference and the members instead of the synthetic one (prepare_data). Returns the JSON record."""
+	ltc_dir: LTC table for the reference and the members instead of the synthetic one; noise_root: Ahmed-Wonka table for the reference and the
+	members instead of white noise (prepare_data). Returns the JSON record."""
 	from . import convergence
-	from .frame import Frame
 	by_name = {e["name"]: e for e in experiment_list(all_timings=False)}
 
 	def open_frame(experiment):
-		info = prepare_data(experiment, data_root, ltc_dir)
-		frame = Frame(info["vks"], info["textures"], info["save"], info["ltc"], cuda_device=cuda_device)
+		frame = open_dataset_frame(prepare_data(experiment, data_root, ltc_dir, noise_root), cuda_device)
 		_configure(frame, experiment)
 		return frame
 
@@ -284,6 +296,8 @@ def run_convergence(group, data_root, out_dir, reference_frames, variance_frames
 		reference_mean_variance=list(reference.mean_variance) if reference.mean_variance is not None else None,
 		reference_frame_error=reference_frame_error, accumulate_ms_per_frame=round(reference.accumulate_ms_per_frame, 5), variance_frames=variance_frames,
 		timed="accumulate kernel per frame at %dx%d, CUDA events" % (w, h), members=[])
+	if noise_root is not None:
+		record["noise_root"] = noise_root
 	for name in group["members"]:
 		experiment = by_name[name]
 		frame = open_frame(experiment)

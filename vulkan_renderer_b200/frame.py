@@ -12,7 +12,10 @@ from . import api
 class Frame:
 	"""Owns device, scene, LTC table, noise table and the scene specification of one dataset."""
 
-	def __init__(self, vks, textures, save, ltc_dir, cuda_device=0, stream=None, noise=(256, 256, 64), fresnel_count=51, request_acceleration_structure=True):
+	def __init__(self, vks, textures, save, ltc_dir, cuda_device=0, stream=None, noise=(256, 256, 64), fresnel_count=51, request_acceleration_structure=True,
+		noise_type=api.NOISE_WHITE, noise_root=None):
+		"""noise = (width, height, layers) of the noise table. noise_type api.NOISE_BLUE or api.NOISE_AHMED reads the table from
+		<noise_root>/data/noise/<the loader's file name> (e.g. written by tools/make_noise_tables.py) and uploads it with the loader's initial seed."""
 		self.lib = api.load_library()
 		self.device = api.Device(); self.scene = api.Scene(); self.ltc = api.LtcTable(); self.noise = api.NoiseTable()
 		self.spec = api.SceneSpecification(); self.settings = api.RenderSettings()
@@ -20,7 +23,14 @@ class Frame:
 		self._check(self.lib.vkr_create_device(C.byref(self.device), cuda_device, stream), "vkr_create_device")
 		self._check(self.lib.vkr_load_scene(C.byref(self.scene), C.byref(self.device), vks.encode(), textures.encode(), int(request_acceleration_structure)), "vkr_load_scene")
 		self._check(self.lib.vkr_load_ltc_table(C.byref(self.ltc), C.byref(self.device), ltc_dir.encode(), fresnel_count), "vkr_load_ltc_table")
-		self._check(self.lib.vkr_load_noise_table(C.byref(self.noise), C.byref(self.device), noise[0], noise[1], noise[2], api.NOISE_WHITE), "vkr_load_noise_table")
+		if noise_type == api.NOISE_WHITE:
+			self._check(self.lib.vkr_load_noise_table(C.byref(self.noise), C.byref(self.device), noise[0], noise[1], noise[2], api.NOISE_WHITE), "vkr_load_noise_table")
+		else:
+			from .noise_gen import LOADER_SEED, read_noise_table
+			if noise_root is None:
+				raise ValueError("noise type %d is read from a file: pass noise_root" % noise_type)
+			texels = read_noise_table(noise_root, noise_type, *noise)
+			self._check(self.lib.vkr_noise_table_from_image(C.byref(self.noise), C.byref(self.device), noise[0], noise[1], noise[2], texels.ctypes.data, LOADER_SEED), "vkr_noise_table_from_image")
 		self._check(self.lib.vkr_quick_load(C.byref(self.spec), save.encode()), "vkr_quick_load")
 		# create_and_assign_light_textures (src/main.c:371): texture indices for all lights; the textures go to the device only if a light is textured
 		self.light_textures = api.LightTextures()
