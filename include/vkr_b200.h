@@ -549,6 +549,14 @@ int vkr_trace_shadow_rays(const vkr_device_t* device, const vkr_scene_t* scene, 
 /* ---- sampling probe (tests / KATs): clip + prepare + sample in the polygon's local space on the device */
 int vkr_sample_polygon_batch(const vkr_device_t* device, uint32_t vertex_count, const float* vertices_xyz, int biased,
 	uint32_t n, const float* random_numbers, float* out_dirs, float* out_info);
+/* ---- related-work sampling probe (tests / KATs): the prepare() and sample() of the related-work tile kernel (technique 0..10) for one light and
+        one shading point, one GPU thread per sample. light_block: the light's block of the constant buffer for vertex bound max_vertex_count (3..7),
+        light_block_bytes = 160 + 32 max_vertex_count + 16 (max_vertex_count - 2); world_to_shading: rows x, y, z, then the translation (12 floats).
+        out_dirs: 3 floats per sample (world space), out_densities: per solid angle. *out_lit = 0 if the light is culled: then the GGX density factor is 0
+        and the directions and densities are left as they were. Anything else out of range is refused (return 1) before any allocation or launch. */
+int vkr_sample_related_work_batch(const vkr_device_t* device, uint32_t technique, uint32_t max_vertex_count,
+	const void* light_block, uint32_t light_block_bytes, const float* position, const float* world_to_shading /* 12 */,
+	uint32_t n, const float* random_numbers, float* out_dirs, float* out_densities, float* out_ggx_density_factor, int32_t* out_lit);
 
 /* ---- arithmetic probe: the kernels' reciprocal square root (one range check in front of the square root's and the reciprocal's fast paths, csrc/vkr_device_math.cuh)
         against its definition 1.0f / sqrtf(x) for all 2^32 floats on the device; mismatches must come back 0 */

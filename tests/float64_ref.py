@@ -24,10 +24,11 @@ def _clip_halfspace(poly, normal):
 	return out
 
 
-def lambert_psa(poly):
-	"""Projected solid angle of a spherical polygon in the upper hemisphere (Lambert: half the z-weighted sum of the edges' arc lengths). Edges of
-	length zero (a clip crossing that coincides with a vertex) contribute nothing."""
-	total = 0.0
+def vector_irradiance(poly):
+	"""The integral of the direction w over a spherical polygon (smaller than a hemisphere), half the sum over its edges of the arc length times the
+	edge plane's unit normal (Lambert), oriented towards the polygon. Edges of length zero (a clip crossing that coincides with a vertex) contribute
+	nothing."""
+	total = np.zeros(3)
 	n = len(poly)
 	unit = []
 	for p in poly:
@@ -39,8 +40,28 @@ def lambert_psa(poly):
 		s = math.sqrt(cx * cx + cy * cy + cz * cz)
 		if s == 0.0:
 			continue
-		total += math.atan2(s, a[0] * b[0] + a[1] * b[1] + a[2] * b[2]) * cz / s
-	return abs(0.5 * total)
+		total += math.atan2(s, a[0] * b[0] + a[1] * b[1] + a[2] * b[2]) / s * np.array([cx, cy, cz])
+	total *= 0.5
+	return -total if total @ np.sum(unit, axis=0) < 0.0 else total
+
+
+def lambert_psa(poly):
+	"""Projected solid angle of a spherical polygon in the upper hemisphere: the z component of its vector irradiance."""
+	return abs(float(vector_irradiance(poly)[2]))
+
+
+def solid_angle(poly):
+	"""Solid angle of a convex polygon seen from the origin: a fan of triangles around vertex 0, each by Van Oosterom and Strackee (1983),
+	tan(omega / 2) = |det(a, b, c)| / (|a||b||c| + (a.b)|c| + (b.c)|a| + (c.a)|b|). The determinant is taken over the edges from a, which keeps
+	its relative accuracy for distant specks."""
+	P = np.asarray(poly, dtype=np.float64)
+	r = np.linalg.norm(P, axis=1)
+	total = 0.0
+	for k in range(1, len(P) - 1):
+		a, b, c = P[0], P[k], P[k + 1]
+		det = abs(float(np.dot(a, np.cross(b - a, c - a))))
+		total += 2.0 * math.atan2(det, r[0] * r[k] * r[k + 1] + (a @ b) * r[k + 1] + (b @ c) * r[0] + (c @ a) * r[k])
+	return total
 
 
 def clip_and_psa(pts, horizon_eps=1.0e-6):

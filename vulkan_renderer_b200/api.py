@@ -22,7 +22,7 @@ EXPORTED_SYMBOLS = [
 	"vkr_create_shading_pass", "vkr_destroy_shading_pass", "vkr_shading_pass_run", "vkr_shading_pass_run_host", "vkr_shading_pass_wait", "vkr_shading_pass_run_with_counters",
 	"vkr_create_frame_exchange", "vkr_destroy_frame_exchange", "vkr_frame_exchange_get_handle", "vkr_frame_exchange_connect", "vkr_frame_exchange_connect_local",
 	"vkr_frame_exchange_frame", "vkr_shading_pass_run_exchange", "vkr_shading_pass_run_host_exchange", "vkr_frame_exchange_wait", "vkr_frame_exchange_download",
-	"vkr_trace_shadow_rays", "vkr_sample_polygon_batch", "vkr_probe_rsqrt_exhaustive", "vkr_bvh_build_probe", "vkr_bvh_build_probe_with", "vkr_bvh_build_probe_device", "vkr_bvh4_build_probe", "vkr_bvh_free_probe",
+	"vkr_trace_shadow_rays", "vkr_sample_polygon_batch", "vkr_sample_related_work_batch", "vkr_probe_rsqrt_exhaustive", "vkr_bvh_build_probe", "vkr_bvh_build_probe_with", "vkr_bvh_build_probe_device", "vkr_bvh4_build_probe", "vkr_bvh_free_probe",
 	"vkr_quantize_unorm8", "vkr_combine_ldr_screenshots_into_hdr", "vkr_write_png", "vkr_write_hdr", "vkr_take_screenshot",
 	"vkr_record_frame_time", "vkr_get_frame_time", "vkr_reset_frame_times",
 	"vkr_load_texture", "vkr_destroy_texture", "vkr_texture_from_levels", "vkr_scene_from_buffers", "vkr_ltc_table_from_images", "vkr_noise_table_from_image", "vkr_create_and_assign_light_textures", "vkr_destroy_light_textures",
@@ -235,6 +235,7 @@ def load_library():
 	lib.vkr_frame_exchange_download.argtypes = [P(FrameExchange), P(Device), C.c_void_p]
 	lib.vkr_trace_shadow_rays.argtypes = [P(Device), P(Scene), C.c_uint32, C.c_void_p, C.c_void_p]
 	lib.vkr_sample_polygon_batch.argtypes = [P(Device), C.c_uint32, C.c_void_p, C.c_int, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
+	lib.vkr_sample_related_work_batch.argtypes = [P(Device), C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, P(C.c_float), P(C.c_int32)]
 	lib.vkr_probe_rsqrt_exhaustive.argtypes = [P(Device), P(C.c_uint64), P(C.c_uint32)]
 	lib.vkr_bvh_build_probe.argtypes = [C.c_void_p, C.c_uint64, P(P(C.c_float)), P(C.c_uint64), P(P(C.c_float)), P(P(C.c_uint32)), P(C.c_uint32)]
 	lib.vkr_bvh_build_probe_with.argtypes = [C.c_int, C.c_void_p, C.c_uint64, P(P(C.c_float)), P(C.c_uint64), P(P(C.c_float)), P(P(C.c_uint32)), P(C.c_uint32)]

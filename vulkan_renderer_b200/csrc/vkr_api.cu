@@ -514,3 +514,46 @@ extern "C" int vkr_sample_polygon_batch(const vkr_device_t* device, uint32_t ver
 	VKR_CUDA_OK(err2, "The sampling probe failed");
 	return 0;
 }
+
+extern "C" int vkr_sample_related_work_batch(const vkr_device_t* device, uint32_t technique, uint32_t max_vertex_count, const void* light_block, uint32_t light_block_bytes,
+	const float* position, const float* world_to_shading, uint32_t n, const float* random_numbers, float* out_dirs, float* out_densities, float* out_ggx_density_factor, int32_t* out_lit)
+{
+	if (!device || !light_block || !position || !world_to_shading || !out_ggx_density_factor || !out_lit || (n && (!random_numbers || !out_dirs || !out_densities))) {
+		printf("The related-work sampling probe needs a device, a light block, a position, a frame and its outputs.\n"); return 1;
+	}
+	if (technique > 10) { printf("The related-work sampling probe supports techniques 0 to 10.\n"); return 1; }
+	if (max_vertex_count < 3 || max_vertex_count > 7) { printf("The related-work sampling probe supports vertex bounds 3 to 7.\n"); return 1; }
+	if (light_block_bytes != 160 + 32 * max_vertex_count + 16 * (max_vertex_count - 2)) { printf("The light block of vertex bound %u has %u bytes.\n", max_vertex_count, 160 + 32 * max_vertex_count + 16 * (max_vertex_count - 2)); return 1; }
+	vkr_related_work_probe_launcher_t* const launchers[5] = { vkr_launch_related_work_probe_v3, vkr_launch_related_work_probe_v4, vkr_launch_related_work_probe_v5, vkr_launch_related_work_probe_v6, vkr_launch_related_work_probe_v7 };
+	VKR_CUDA_OK(cudaSetDevice(device->cuda_device), "Failed to select the CUDA device");
+	cudaStream_t stream = (cudaStream_t) device->stream;
+	const size_t nn = n ? n : 1;
+	unsigned char* d_light = nullptr; float *d_pf = nullptr, *d_r = nullptr, *d_d = nullptr, *d_p = nullptr, *d_g = nullptr;
+	auto release = [&]() { cudaFree(d_light); cudaFree(d_pf); cudaFree(d_r); cudaFree(d_d); cudaFree(d_p); cudaFree(d_g); };
+	if (cudaMalloc(&d_light, light_block_bytes) != cudaSuccess || cudaMalloc(&d_pf, sizeof(float) * 15) != cudaSuccess || cudaMalloc(&d_r, sizeof(float) * 2 * nn) != cudaSuccess
+		|| cudaMalloc(&d_d, sizeof(float) * 3 * nn) != cudaSuccess || cudaMalloc(&d_p, sizeof(float) * nn) != cudaSuccess || cudaMalloc(&d_g, sizeof(float) * 2) != cudaSuccess)
+	{
+		release(); printf("Failed to allocate buffers for the related-work sampling probe.\n"); return 1;
+	}
+	if (cudaMemcpyAsync(d_light, light_block, light_block_bytes, cudaMemcpyHostToDevice, stream) != cudaSuccess
+		|| cudaMemcpyAsync(d_pf, position, sizeof(float) * 3, cudaMemcpyHostToDevice, stream) != cudaSuccess
+		|| cudaMemcpyAsync(d_pf + 3, world_to_shading, sizeof(float) * 12, cudaMemcpyHostToDevice, stream) != cudaSuccess
+		|| (n && cudaMemcpyAsync(d_r, random_numbers, sizeof(float) * 2 * (size_t) n, cudaMemcpyHostToDevice, stream) != cudaSuccess))
+	{
+		release(); printf("Failed to upload the inputs of the related-work sampling probe.\n"); return 1;
+	}
+	const cudaError_t err = launchers[max_vertex_count - 3](technique, d_light, d_pf, n, d_r, d_d, d_p, d_g, stream);
+	float ggx_lit[2] = { 0.0f, 0.0f };
+	cudaMemcpyAsync(ggx_lit, d_g, sizeof(ggx_lit), cudaMemcpyDeviceToHost, stream);
+	cudaError_t err2 = cudaStreamSynchronize(stream);
+	if (err == cudaSuccess && err2 == cudaSuccess && ggx_lit[1] != 0.0f && n) { // a culled light leaves the directions and densities as they were
+		cudaMemcpyAsync(out_dirs, d_d, sizeof(float) * 3 * (size_t) n, cudaMemcpyDeviceToHost, stream);
+		cudaMemcpyAsync(out_densities, d_p, sizeof(float) * (size_t) n, cudaMemcpyDeviceToHost, stream);
+		err2 = cudaStreamSynchronize(stream);
+	}
+	release();
+	VKR_CUDA_OK(err, "Failed to launch the related-work sampling probe");
+	VKR_CUDA_OK(err2, "The related-work sampling probe failed");
+	*out_ggx_density_factor = ggx_lit[0]; *out_lit = ggx_lit[1] != 0.0f ? 1 : 0;
+	return 0;
+}

@@ -75,6 +75,11 @@ vkr_tile_launcher_t vkr_launch_shading_kernel_stats_v4;
 vkr_tile_launcher_t vkr_launch_textured_light_kernel_v3, vkr_launch_textured_light_kernel_v4, vkr_launch_textured_light_kernel_v5, vkr_launch_textured_light_kernel_v6, vkr_launch_textured_light_kernel_v7;
 // vkr_related_work_kernel.cu: the related-work sampling techniques and the error display
 vkr_tile_launcher_t vkr_launch_related_work_kernel_v3, vkr_launch_related_work_kernel_v4, vkr_launch_related_work_kernel_v5, vkr_launch_related_work_kernel_v6, vkr_launch_related_work_kernel_v7;
+// and the sampling probe of the same samplers (vkr_sample_related_work_batch), one thread per sample. All pointers are device pointers;
+// position_frame = 3 + 12 floats, out_ggx_lit = {GGX density factor, 1 if lit else 0}.
+typedef cudaError_t vkr_related_work_probe_launcher_t(uint32_t technique, const unsigned char* light_block, const float* position_frame, uint32_t n, const float* random_numbers,
+	float* out_dirs, float* out_densities, float* out_ggx_lit, cudaStream_t stream);
+vkr_related_work_probe_launcher_t vkr_launch_related_work_probe_v3, vkr_launch_related_work_probe_v4, vkr_launch_related_work_probe_v5, vkr_launch_related_work_probe_v6, vkr_launch_related_work_probe_v7;
 // vkr_textured_related_work_kernel.cu: the related-work sampling techniques for frames with textured lights
 vkr_tile_launcher_t vkr_launch_textured_related_work_kernel_v3, vkr_launch_textured_related_work_kernel_v4, vkr_launch_textured_related_work_kernel_v5, vkr_launch_textured_related_work_kernel_v6, vkr_launch_textured_related_work_kernel_v7;
 // float node pairs -> quantised node pairs (vkr_lbvh_gpu.cu); d_nodes_q: 32 bytes per pair

@@ -38,9 +38,44 @@ related_work_kernel(const shading_kernel_params p) {
 	shade_tile<MAXV + 1, false, TRACE>(p, related_work_light_shader<STRATEGY, MAXV, TRACE>());
 }
 
+// Sampling probe (vkr_sample_related_work_batch): one thread per sample runs the prepare() and sample() of the tile kernel's light shader for one
+// (light, shading point) pair. frame = rows x, y, z of world_to_shading_space, then its translation. Thread 0 writes the GGX density factor and
+// whether the light is lit; a culled light leaves the directions and densities as they were.
+template <int TECHNIQUE, int MAXV>
+__global__ void __launch_bounds__(128)
+related_work_probe_kernel(const unsigned char* light_block, const float* position_frame, uint32_t n, const float* rnd, float* out_dirs, float* out_densities, float* out_ggx_lit) {
+	rw_light<MAXV> light;
+	rw_load_light<MAXV>(light, light_block);
+	const float* fr = position_frame + 3;
+	rw_frame frame;
+	frame.rx = make3(fr[0], fr[1], fr[2]); frame.ry = make3(fr[3], fr[4], fr[5]); frame.rz = make3(fr[6], fr[7], fr[8]); frame.t = make3(fr[9], fr[10], fr[11]);
+	rw_sampler<TECHNIQUE, MAXV> sampler;
+	const bool lit = sampler.prepare(light, make3(position_frame[0], position_frame[1], position_frame[2]), frame);
+	const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i == 0) { out_ggx_lit[0] = lit ? sampler.ggx_density_factor() : 0.0f; out_ggx_lit[1] = lit ? 1.0f : 0.0f; }
+	if (i >= n || !lit) return;
+	float density;
+	const f3 d = sampler.sample(make2(rnd[2 * i], rnd[2 * i + 1]), &density);
+	out_dirs[3 * i] = d.x; out_dirs[3 * i + 1] = d.y; out_dirs[3 * i + 2] = d.z;
+	out_densities[i] = density;
+}
+
 } // namespace vkr
 
 using namespace vkr;
+
+cudaError_t VKR_TILE_LAUNCHER(vkr_launch_related_work_probe_v)(uint32_t technique, const unsigned char* light_block, const float* position_frame, uint32_t n, const float* random_numbers,
+	float* out_dirs, float* out_densities, float* out_ggx_lit, cudaStream_t stream)
+{
+	const unsigned blocks = (n + 127) / 128 > 0 ? (n + 127) / 128 : 1;
+	switch (technique) {
+#define VKR_PROBE(T) case T: related_work_probe_kernel<T, VKR_MAXV_TU><<<blocks, 128, 0, stream>>>(light_block, position_frame, n, random_numbers, out_dirs, out_densities, out_ggx_lit); break;
+	VKR_PROBE(0) VKR_PROBE(1) VKR_PROBE(2) VKR_PROBE(3) VKR_PROBE(4) VKR_PROBE(5) VKR_PROBE(6) VKR_PROBE(7) VKR_PROBE(8) VKR_PROBE(9) VKR_PROBE(10)
+#undef VKR_PROBE
+	default: return cudaErrorInvalidValue;
+	}
+	return cudaGetLastError();
+}
 
 cudaError_t VKR_TILE_LAUNCHER(vkr_launch_related_work_kernel_v)(const shading_kernel_params& p, cudaStream_t stream) {
 	if (p.error_display != 0) { // the error display modes of projected solid angle sampling (techniques 10, 11, 12)
