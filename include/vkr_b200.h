@@ -415,6 +415,9 @@ typedef struct vkr_shading_pass_s {
 	void* d_tile_cost; void* h_tile_cost;
 	void* event_costs; int costs_pending;
 	int reorder_tiles;
+	/* the tile list of vkr_shading_pass_run_tiles (tile_count entries each, allocated at its first call); event_subset: recorded after its upload */
+	void* d_subset_tiles; void* h_subset_tiles;
+	void* event_subset;
 } vkr_shading_pass_t;
 
 int vkr_create_shading_pass(vkr_shading_pass_t* pass, const vkr_device_t* device, const vkr_shading_pass_desc_t* desc);
@@ -425,6 +428,11 @@ void vkr_destroy_shading_pass(vkr_shading_pass_t* pass, const vkr_device_t* devi
 int vkr_shading_pass_run(vkr_shading_pass_t* pass, const vkr_device_t* device, const void* constants, size_t constants_size, const void* d_gbuffer, void* d_out_rgba32f);
 /* End-to-end variant with HOST buffers: uploads the G-buffer tiles of this instance, shades, downloads them, waits. */
 int vkr_shading_pass_run_host(vkr_shading_pass_t* pass, const vkr_device_t* device, const void* constants, size_t constants_size, const float* gbuffer, float* out_rgba32f);
+/* Asynchronous like vkr_shading_pass_run, but shades only the tiles in tiles[0 .. tile_count) (HOST array of tile indices ty * tiles_x + tx, launched in
+   that order) and writes no other pixel. The pass's own launch order, cost readback and reorder_tiles are left as they are. Refuses an index out of
+   range, a tile outside this instance's share and a repeated tile; an empty list launches nothing. */
+int vkr_shading_pass_run_tiles(vkr_shading_pass_t* pass, const vkr_device_t* device, const void* constants, size_t constants_size, const void* d_gbuffer, void* d_out_rgba32f,
+	const uint32_t* tiles, uint32_t tile_count);
 int vkr_shading_pass_wait(vkr_shading_pass_t* pass, const vkr_device_t* device);
 
 /* ---- one frame on several GPUs (replaces nothing in the reference, which drives one GPU; SURVEY 8e). Every GPU of the box runs its
@@ -543,6 +551,43 @@ typedef struct vkr_frame_error_s {
 } vkr_frame_error_t;
 /* synchronous; both frames are DEVICE pointers to width*height float4 */
 int vkr_compare_frames(const vkr_device_t* device, uint32_t width, uint32_t height, const void* d_frame_rgba32f, const void* d_reference_rgba32f, vkr_frame_error_t* out);
+
+/* ---- adaptive accumulation: the accumulator above per 16x8 screen tile (VKR_TILE_WIDTH x VKR_TILE_ROW_HEIGHT, edge tiles clipped; tile
+        ty * tiles_x + tx), so that a converged reference stops shading the tiles whose mean has converged. Each tile has a frame count n_t and an
+        active flag; after create / reset every tile is active with n_t = 0. A frame updates the pixels of the active tiles only, with n = n_t + 1
+        (the rule of vkr_accumulate_frame), so a tile's state is the plain accumulator's after its first n_t frames. The tile test
+        (vkr_adaptive_update_tiles) stops a tile when n_t >= max_frames, or when n_t >= min_frames and every pixel and channel has
+        v <= target_rel_mse * (mean^2 + 0.01), v = m2 / (n_t (n_t - 1)) the estimated variance of the mean (0.01: the relMSE epsilon of
+        vkr_compare_frames); NaN or infinity keeps a tile active. A stopped tile never becomes active again. float64, fixed order of every sum
+        (csrc/vkr_accumulate.cuh): bit-identical from call to call and from device to device. Pair it with vkr_shading_pass_run_tiles, which shades
+        the listed tiles only. */
+typedef struct vkr_adaptive_accumulator_s {
+	uint32_t width, height;
+	uint32_t tiles_x, tiles_y;
+	uint64_t frame_count;          /* frames accumulated since create / reset; every active tile has taken each of them */
+	uint32_t active_tile_count;    /* as of the last reset or vkr_adaptive_update_tiles */
+	void* d_state;                 /* 6 planes of width*height double: mean rgb, m2 rgb (Welford) */
+	void* d_tile_frames;           /* uint32 n_t per tile */
+	void* d_tile_active;           /* uint8 per tile, 1 = active */
+	void* d_partials; void* h_partials;   /* reduction scratch, pinned host copy */
+} vkr_adaptive_accumulator_t;
+int vkr_create_adaptive_accumulator(vkr_adaptive_accumulator_t* accumulator, const vkr_device_t* device, uint32_t width, uint32_t height);
+void vkr_destroy_adaptive_accumulator(vkr_adaptive_accumulator_t* accumulator, const vkr_device_t* device);
+/* frame_count = 0, every tile active with n_t = 0 */
+int vkr_adaptive_accumulator_reset(vkr_adaptive_accumulator_t* accumulator, const vkr_device_t* device);
+/* d_frame_rgba32f: DEVICE pointer, width*height float4 (16-byte aligned). The caller guarantees that it holds freshly shaded pixels for every active
+   tile; the pixels of the other tiles are not read. */
+int vkr_adaptive_accumulate_frame(vkr_adaptive_accumulator_t* accumulator, const vkr_device_t* device, const void* d_frame_rgba32f);
+/* Synchronous: the tile test, then the flags to HOST memory. out_active: tiles_x * tiles_y bytes (1 = still active) or NULL; out_active_count may be NULL.
+   Refuses a target that is negative or not finite, min_frames < 2 and max_frames < min_frames. */
+int vkr_adaptive_update_tiles(vkr_adaptive_accumulator_t* accumulator, const vkr_device_t* device, double target_rel_mse, uint32_t min_frames, uint32_t max_frames,
+	uint8_t* out_active, uint32_t* out_active_count);
+/* Synchronous: n_t of every tile to HOST memory (tiles_x * tiles_y uint32) */
+int vkr_adaptive_tile_frames(const vkr_adaptive_accumulator_t* accumulator, const vkr_device_t* device, uint32_t* out_tile_frames);
+/* as vkr_accumulator_resolve, each pixel with its own tile's n_t: the mean (alpha 1) and the per-frame sample variance m2 / (n_t - 1) (alpha 0) */
+int vkr_adaptive_resolve(const vkr_adaptive_accumulator_t* accumulator, const vkr_device_t* device, void* d_mean_rgba32f, void* d_variance_rgba32f);
+/* synchronous: the estimated relMSE of the mean, per channel the mean over all pixels of v / (mean^2 + 0.01), v as in the tile test. frame_count >= 2. */
+int vkr_adaptive_estimated_rel_mse(const vkr_adaptive_accumulator_t* accumulator, const vkr_device_t* device, double out_rel_mse[3]);
 
 /* ---- shadow-ray probe (tests / KATs): rays = {ox,oy,oz,dx,dy,dz,tmin,tmax} per ray on the HOST, out = 1 byte per ray */
 int vkr_trace_shadow_rays(const vkr_device_t* device, const vkr_scene_t* scene, uint32_t ray_count, const float* rays, uint8_t* out_occluded);

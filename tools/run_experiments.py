@@ -2,11 +2,14 @@
 """Runs the reference's experiment list (src/experiment_list.c) on the CUDA path and writes the timing matrix as JSON.
 
   python tools/run_experiments.py --out gpurun_out/experiments [--select timings_central_4] [--width 1920 --height 1080] [--frames 12] [--no-screenshots]
-      [--convergence M [--variance-frames K]] [--ltc DIR] [--noise ROOT]
+      [--convergence M [--variance-frames K] [--adaptive TARGET]] [--ltc DIR] [--noise ROOT]
 
 --convergence M also measures the error of the selected figure experiments against converged references (M animated frames of each reference's
 settings averaged on the device) and their noise level (mean per-frame variance over K animated frames), and writes convergence.json next to
 timings.json (experiments.convergence_groups, experiments.run_convergence).
+
+--adaptive TARGET builds each reference adaptively (convergence.accumulate_adaptive, max_frames = M): a 16x8 tile stops being shaded once every pixel's
+estimated variance of the mean is at most TARGET * (mean^2 + 0.01); convergence.json then also holds what each reference shaded and its estimated relMSE.
 
 --ltc DIR shades every experiment with the LTC table in DIR (fit<i>.dat, e.g. written by tools/fit_ltc.py) instead of the datasets' synthetic one.
 
@@ -35,6 +38,7 @@ def main():
 	ap.add_argument("--no-figs", action="store_true"); ap.add_argument("--no-timings", action="store_true"); ap.add_argument("--no-screenshots", action="store_true")
 	ap.add_argument("--convergence", type=int, default=0, metavar="M", help="frames averaged into each reference; 0: no convergence measurement")
 	ap.add_argument("--variance-frames", type=int, default=16, metavar="K", help="animated frames per member for its mean variance (with --convergence)")
+	ap.add_argument("--adaptive", type=float, default=None, metavar="TARGET", help="build the references adaptively to this relMSE target (with --convergence)")
 	ap.add_argument("--ltc", default=None, metavar="DIR", help="directory of fit<i>.dat files to shade with instead of the synthetic LTC table")
 	ap.add_argument("--noise", default=None, metavar="ROOT", help="directory holding data/noise/ahmed_2d_rgba_256x256_64.blob to shade with instead of white noise")
 	args = ap.parse_args()
@@ -48,7 +52,7 @@ def main():
 		groups = [g for g in groups if g["members"]]
 		print("%d convergence groups" % len(groups))
 		experiments.run_convergences(groups, args.data, args.out, os.path.join(args.out, "convergence.json"), args.convergence, args.variance_frames,
-			width=args.width, height=args.height, ltc_dir=args.ltc, noise_root=args.noise)
+			width=args.width, height=args.height, ltc_dir=args.ltc, noise_root=args.noise, adaptive=args.adaptive)
 
 
 if __name__ == "__main__":

@@ -19,7 +19,7 @@ EXPORTED_SYMBOLS = [
 	"vkr_get_world_to_projection_space", "vkr_quick_load", "vkr_quick_save", "vkr_destroy_scene_specification",
 	"vkr_specify_default_render_settings", "vkr_get_constants_size", "vkr_write_constants", "vkr_set_frame_bits",
 	"vkr_gbuffer_size", "vkr_run_visibility_pass", "vkr_run_gbuffer_pass",
-	"vkr_create_shading_pass", "vkr_destroy_shading_pass", "vkr_shading_pass_run", "vkr_shading_pass_run_host", "vkr_shading_pass_wait", "vkr_shading_pass_run_with_counters",
+	"vkr_create_shading_pass", "vkr_destroy_shading_pass", "vkr_shading_pass_run", "vkr_shading_pass_run_host", "vkr_shading_pass_wait", "vkr_shading_pass_run_with_counters", "vkr_shading_pass_run_tiles",
 	"vkr_create_frame_exchange", "vkr_destroy_frame_exchange", "vkr_frame_exchange_get_handle", "vkr_frame_exchange_connect", "vkr_frame_exchange_connect_local",
 	"vkr_frame_exchange_frame", "vkr_shading_pass_run_exchange", "vkr_shading_pass_run_host_exchange", "vkr_frame_exchange_wait", "vkr_frame_exchange_download",
 	"vkr_trace_shadow_rays", "vkr_sample_polygon_batch", "vkr_sample_related_work_batch", "vkr_probe_rsqrt_exhaustive", "vkr_bvh_build_probe", "vkr_bvh_build_probe_with", "vkr_bvh_build_probe_device", "vkr_bvh4_build_probe", "vkr_bvh_free_probe",
@@ -28,6 +28,8 @@ EXPORTED_SYMBOLS = [
 	"vkr_load_texture", "vkr_destroy_texture", "vkr_texture_from_levels", "vkr_scene_from_buffers", "vkr_ltc_table_from_images", "vkr_noise_table_from_image", "vkr_create_and_assign_light_textures", "vkr_destroy_light_textures",
 	"vkr_create_render_targets", "vkr_destroy_render_targets", "vkr_download_frame", "vkr_download_gbuffer", "vkr_upload_gbuffer",
 	"vkr_create_accumulator", "vkr_destroy_accumulator", "vkr_accumulator_reset", "vkr_accumulate_frame", "vkr_accumulator_resolve", "vkr_accumulator_mean_variance", "vkr_compare_frames",
+	"vkr_create_adaptive_accumulator", "vkr_destroy_adaptive_accumulator", "vkr_adaptive_accumulator_reset", "vkr_adaptive_accumulate_frame", "vkr_adaptive_update_tiles",
+	"vkr_adaptive_tile_frames", "vkr_adaptive_resolve", "vkr_adaptive_estimated_rel_mse",
 	"vkr_ltc_fit_default_desc", "vkr_fit_ltc_table", "vkr_write_ltc_fits",
 	"vkr_noise_gen_default_desc", "vkr_generate_noise_table", "vkr_write_noise_table",
 ]
@@ -128,7 +130,8 @@ class ShadingPass(C.Structure):
 		("d_gbuffer_staging", C.c_void_p), ("d_out_staging", C.c_void_p), ("kernel_launches", C.c_uint64), ("last_kernel_ms", C.c_float),
 		("event_begin", C.c_void_p), ("event_end", C.c_void_p), ("timing_enabled", C.c_int),
 		("event_constants", C.c_void_p), ("tile_count", C.c_uint32), ("d_tile_list", C.c_void_p), ("h_tile_list", C.c_void_p),
-		("d_tile_cost", C.c_void_p), ("h_tile_cost", C.c_void_p), ("event_costs", C.c_void_p), ("costs_pending", C.c_int), ("reorder_tiles", C.c_int)]
+		("d_tile_cost", C.c_void_p), ("h_tile_cost", C.c_void_p), ("event_costs", C.c_void_p), ("costs_pending", C.c_int), ("reorder_tiles", C.c_int),
+		("d_subset_tiles", C.c_void_p), ("h_subset_tiles", C.c_void_p), ("event_subset", C.c_void_p)]
 
 
 MAX_GPUS = 8   # VKR_MAX_GPUS
@@ -143,6 +146,12 @@ class FrameExchange(C.Structure):
 class Accumulator(C.Structure):
 	"""vkr_accumulator_t: running mean and sum of squared deviations of frames, float64 (include/vkr_b200.h)."""
 	_fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("frame_count", C.c_uint64), ("d_state", C.c_void_p), ("d_partials", C.c_void_p), ("h_partials", C.c_void_p)]
+
+
+class AdaptiveAccumulator(C.Structure):
+	"""vkr_adaptive_accumulator_t: the accumulator's state per 16x8 screen tile, with a frame count and an active flag per tile (include/vkr_b200.h)."""
+	_fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("tiles_x", C.c_uint32), ("tiles_y", C.c_uint32), ("frame_count", C.c_uint64), ("active_tile_count", C.c_uint32),
+		("d_state", C.c_void_p), ("d_tile_frames", C.c_void_p), ("d_tile_active", C.c_void_p), ("d_partials", C.c_void_p), ("h_partials", C.c_void_p)]
 
 
 class FrameError(C.Structure):
@@ -222,6 +231,7 @@ def load_library():
 	lib.vkr_shading_pass_run.argtypes = [P(ShadingPass), P(Device), C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
 	lib.vkr_shading_pass_run_host.argtypes = [P(ShadingPass), P(Device), C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]
 	lib.vkr_shading_pass_wait.argtypes = [P(ShadingPass), P(Device)]
+	lib.vkr_shading_pass_run_tiles.argtypes = [P(ShadingPass), P(Device), C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]
 	lib.vkr_shading_pass_run_with_counters.argtypes = [P(ShadingPass), P(Device), C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, P(C.c_uint64)]
 	lib.vkr_create_frame_exchange.argtypes = [P(FrameExchange), P(Device), C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]
 	lib.vkr_destroy_frame_exchange.argtypes = [P(FrameExchange), P(Device)]; lib.vkr_destroy_frame_exchange.restype = None
@@ -266,6 +276,14 @@ def load_library():
 	lib.vkr_accumulator_resolve.argtypes = [P(Accumulator), P(Device), C.c_void_p, C.c_void_p]
 	lib.vkr_accumulator_mean_variance.argtypes = [P(Accumulator), P(Device), P(C.c_double)]
 	lib.vkr_compare_frames.argtypes = [P(Device), C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, P(FrameError)]
+	lib.vkr_create_adaptive_accumulator.argtypes = [P(AdaptiveAccumulator), P(Device), C.c_uint32, C.c_uint32]
+	lib.vkr_destroy_adaptive_accumulator.argtypes = [P(AdaptiveAccumulator), P(Device)]; lib.vkr_destroy_adaptive_accumulator.restype = None
+	lib.vkr_adaptive_accumulator_reset.argtypes = [P(AdaptiveAccumulator), P(Device)]
+	lib.vkr_adaptive_accumulate_frame.argtypes = [P(AdaptiveAccumulator), P(Device), C.c_void_p]
+	lib.vkr_adaptive_update_tiles.argtypes = [P(AdaptiveAccumulator), P(Device), C.c_double, C.c_uint32, C.c_uint32, C.c_void_p, P(C.c_uint32)]
+	lib.vkr_adaptive_tile_frames.argtypes = [P(AdaptiveAccumulator), P(Device), C.c_void_p]
+	lib.vkr_adaptive_resolve.argtypes = [P(AdaptiveAccumulator), P(Device), C.c_void_p, C.c_void_p]
+	lib.vkr_adaptive_estimated_rel_mse.argtypes = [P(AdaptiveAccumulator), P(Device), P(C.c_double)]
 	lib.vkr_ltc_fit_default_desc.argtypes = [P(LtcFitDesc)]; lib.vkr_ltc_fit_default_desc.restype = None
 	lib.vkr_fit_ltc_table.argtypes = [P(Device), P(LtcFitDesc), C.c_void_p, P(LtcFitStats)]
 	lib.vkr_write_ltc_fits.argtypes = [C.c_char_p, C.c_uint32, C.c_uint32, C.c_void_p]

@@ -149,6 +149,71 @@ VKR_ACC_FN void finish_mean_variance(const double* total, double* mean_variance)
 	for (int c = 0; c != 3; ++c) mean_variance[c] = total[c] / total[kSlotCount];
 }
 
+// ---- adaptive accumulation (vkr_adaptive_accumulator_t): the same state planes, plus per 16x8 screen tile (the unit a CTA of the shading pass shades)
+// a frame count n_t and an active flag. Tile t = ty * tiles_x + tx holds the pixels x = 16 tx + k % 16, y = 8 ty + k / 16, k = 0 .. 127, that lie in
+// the frame (edge tiles are clipped). The kernels run one CTA of kTilePixels threads per tile, thread k on pixel k.
+//   Masked accumulate: every pixel of an active tile takes the frame by accumulate_pixel with n = n_t + 1, then n_t += 1; inactive tiles are not touched.
+//   Tile test (target, min_frames, max_frames), per active tile with n = n_t: n >= max_frames -> inactive; else if n >= min_frames and every pixel
+//   passes pixel_converged -> inactive. pixel_converged per channel c = 0, 1, 2 in that order: v = m2 / ((double) n * (double) (n - 1)),
+//   bound = target * (mean * mean + kRelMseEpsilon), pass iff mean and m2 are finite and v <= bound. The conjunction over the pixels is exact,
+//   so its order does not matter. A tile never becomes active again.
+//   Estimated error: per channel the mean over all pixels of v / (mean * mean + kRelMseEpsilon), v with the pixel's own tile's n_t, summed with the
+//   fixed partition, tree and final sum above (slots [0..2] and kSlotCount).
+constexpr int kTileWidth = 16, kTileHeight = 8, kTilePixels = kTileWidth * kTileHeight;   // VKR_TILE_WIDTH x VKR_TILE_ROW_HEIGHT
+
+VKR_ACC_FN uint32_t tiles_across(uint32_t width) { return (width + kTileWidth - 1) / kTileWidth; }
+VKR_ACC_FN uint32_t tiles_down(uint32_t height) { return (height + kTileHeight - 1) / kTileHeight; }
+
+// pixel k of tile `tile` -> its index i; false if that pixel lies outside the frame
+VKR_ACC_FN bool tile_pixel(uint32_t width, uint32_t height, uint32_t tile, int k, uint64_t* i) {
+	const uint32_t tx = tile % tiles_across(width), ty = tile / tiles_across(width);
+	const uint32_t x = tx * kTileWidth + (uint32_t) k % kTileWidth, y = ty * kTileHeight + (uint32_t) k / kTileWidth;
+	if (x >= width || y >= height) return false;
+	*i = (uint64_t) y * width + x;
+	return true;
+}
+
+VKR_ACC_FN uint32_t pixel_tile(uint32_t width, uint64_t i) {
+	return (uint32_t) (i / width) / kTileHeight * tiles_across(width) + (uint32_t) (i % width) / kTileWidth;
+}
+
+// the estimated variance of the mean of n frames (n >= 2)
+VKR_ACC_FN double variance_of_mean(double m2, uint32_t n) { return m2 / ((double) n * (double) (n - 1)); }
+
+VKR_ACC_FN bool pixel_converged(const double* state, uint64_t plane, uint64_t i, uint32_t n, double target) {
+	bool pass = true;
+	for (int c = 0; c != 3; ++c) {
+		const double mean = state[c * plane + i], m2 = state[(3 + c) * plane + i];
+		const double v = variance_of_mean(m2, n);
+		const double bound = target * (mean * mean + kRelMseEpsilon);
+		pass = pass && finite_value(mean) && finite_value(m2) && v <= bound;
+	}
+	return pass;
+}
+
+// whether the pixels of an active tile with n frames have to be tested at all (they are read only then, and only then is n >= 2)
+VKR_ACC_FN bool tile_needs_test(uint32_t n, uint32_t min_frames, uint32_t max_frames) { return n >= min_frames && n < max_frames; }
+
+// the tile test's outcome for an active tile; converged: every pixel passed pixel_converged (looked at only if tile_needs_test)
+VKR_ACC_FN bool tile_stays_active(uint32_t n, bool converged, uint32_t min_frames, uint32_t max_frames) {
+	if (n >= max_frames) return false;
+	return !(tile_needs_test(n, min_frames, max_frames) && converged);
+}
+
+VKR_ACC_FN void add_estimate_terms(double* t, const double* state, uint64_t plane, uint64_t i, uint32_t n) {
+	for (int c = 0; c != 3; ++c) {
+		const double mean = state[c * plane + i];
+		t[c] = t[c] + variance_of_mean(state[(3 + c) * plane + i], n) / (mean * mean + kRelMseEpsilon);
+	}
+	t[kSlotCount] = t[kSlotCount] + 1.0;
+}
+
+VKR_ACC_FN void thread_estimate_terms(double* t, const double* state, const uint32_t* tile_frames, uint32_t width, uint64_t pixels, int block, int thread) {
+	zero_terms(t);
+	const uint64_t end = partition_end(pixels, block);
+	for (uint64_t i = partition_begin(pixels, block) + (uint64_t) thread; i < end; i += kReduceThreads) add_estimate_terms(t, state, pixels, i, tile_frames[pixel_tile(width, i)]);
+}
+
 // ---- the reductions as one CPU thread runs them: the same blocks, threads, tree and final sum as the kernels (host builds only)
 #ifndef __CUDACC__
 template <class ThreadTerms> inline void reduce_on_host(double* total, ThreadTerms thread_terms) {

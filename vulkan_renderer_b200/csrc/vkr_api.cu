@@ -81,6 +81,9 @@ extern "C" void vkr_destroy_shading_pass(vkr_shading_pass_t* pass, const vkr_dev
 	if (pass->event_end) cudaEventDestroy((cudaEvent_t) pass->event_end);
 	if (pass->event_constants) cudaEventDestroy((cudaEvent_t) pass->event_constants);
 	if (pass->event_costs) cudaEventDestroy((cudaEvent_t) pass->event_costs);
+	if (pass->event_subset) cudaEventDestroy((cudaEvent_t) pass->event_subset);
+	if (pass->d_subset_tiles) cudaFree(pass->d_subset_tiles);
+	if (pass->h_subset_tiles) cudaFreeHost(pass->h_subset_tiles);
 	if (pass->d_tile_list) cudaFree(pass->d_tile_list);
 	if (pass->h_tile_list) cudaFreeHost(pass->h_tile_list);
 	if (pass->d_tile_cost) cudaFree(pass->d_tile_cost);
@@ -204,9 +207,11 @@ cudaError_t vkr_launch_shading_kernel(const vkr::shading_kernel_params& p, cudaS
 	return kTileLaunchers[family][p.max_light_vertex_count - 3](p, stream);
 }
 
-// exchange: when not null, the pixels also go into the frames of the other GPUs (vkr_exchange.cu fills peer_outs)
+// exchange: when not null, the pixels also go into the frames of the other GPUs (vkr_exchange.cu fills peer_outs).
+// subset: when not null, the subset_count tiles listed there (checked by vkr_shading_pass_run_tiles) instead of the pass's own list; the launch order,
+// cost readback and reorder state of the pass stay as they are.
 int vkr_launch_shading(vkr_shading_pass_t* pass, const vkr_device_t* device, const void* constants, size_t constants_size, const void* d_gbuffer, void* d_out, unsigned long long* d_stats,
-	int peer_count, void* const* peer_outs)
+	int peer_count, void* const* peer_outs, const uint32_t* subset, uint32_t subset_count)
 {
 	const vkr_shading_pass_desc_t& d = pass->desc;
 	if (constants_size != pass->constants_size) {
@@ -252,14 +257,21 @@ int vkr_launch_shading(vkr_shading_pass_t* pass, const vkr_device_t* device, con
 	p.width = (int) d.width; p.height = (int) d.height;
 	p.tile_count = (int) pass->tile_count;
 	const bool whole_frame = d.stripe_count == 1;
-	if (pass->reorder_tiles && pass->costs_pending && cudaEventQuery((cudaEvent_t) pass->event_costs) == cudaSuccess) {
+	if (subset) { // the list goes through its own pinned staging, which the previous subset's upload may still be reading
+		VKR_CUDA_OK(cudaEventSynchronize((cudaEvent_t) pass->event_subset), "Failed to wait for the previous upload of a tile list");
+		memcpy(pass->h_subset_tiles, subset, sizeof(uint32_t) * subset_count);
+		VKR_CUDA_OK(cudaMemcpyAsync(pass->d_subset_tiles, pass->h_subset_tiles, sizeof(uint32_t) * subset_count, cudaMemcpyHostToDevice, stream), "Failed to upload the tile list");
+		VKR_CUDA_OK(cudaEventRecord((cudaEvent_t) pass->event_subset, stream), "Failed to record the upload of the tile list");
+		p.tile_count = (int) subset_count;
+	}
+	else if (pass->reorder_tiles && pass->costs_pending && cudaEventQuery((cudaEvent_t) pass->event_costs) == cudaSuccess) {
 		// the costs of an earlier frame are here: new launch order. The list's last upload ran before that frame's kernel, so the staging buffer is free.
 		pass->costs_pending = 0;
 		reorder_tiles_by_cost(pass);
 		VKR_CUDA_OK(cudaMemcpyAsync(pass->d_tile_list, pass->h_tile_list, sizeof(uint32_t) * pass->tile_count, cudaMemcpyHostToDevice, stream), "Failed to upload the tile order");
 	}
-	p.tile_list = (whole_frame && !pass->reorder_tiles) ? nullptr : (const uint32_t*) pass->d_tile_list;
-	const bool record_costs = pass->reorder_tiles && !pass->costs_pending && !d_stats;
+	p.tile_list = subset ? (const uint32_t*) pass->d_subset_tiles : (whole_frame && !pass->reorder_tiles) ? nullptr : (const uint32_t*) pass->d_tile_list;
+	const bool record_costs = pass->reorder_tiles && !pass->costs_pending && !d_stats && !subset;
 	if (record_costs) {
 		const size_t cost_bytes = sizeof(uint32_t) * (size_t) ((d.width + VKR_TILE_WIDTH - 1) / VKR_TILE_WIDTH) * ((d.height + VKR_TILE_ROW_HEIGHT - 1) / VKR_TILE_ROW_HEIGHT);
 		VKR_CUDA_OK(cudaMemsetAsync(pass->d_tile_cost, 0, cost_bytes, stream), "Failed to clear the tile costs");
@@ -316,7 +328,7 @@ int vkr_launch_shading(vkr_shading_pass_t* pass, const vkr_device_t* device, con
 }
 
 static int launch_shading(vkr_shading_pass_t* pass, const vkr_device_t* device, const void* constants, size_t constants_size, const void* d_gbuffer, void* d_out, unsigned long long* d_stats = nullptr) {
-	return vkr_launch_shading(pass, device, constants, constants_size, d_gbuffer, d_out, d_stats, 0, nullptr);
+	return vkr_launch_shading(pass, device, constants, constants_size, d_gbuffer, d_out, d_stats, 0, nullptr, nullptr, 0);
 }
 
 // First tile column of this instance in band `band` (VKR_TILE_BAND_ROWS tile rows): column tx of the band belongs to instance (tx + band) % stripe_count.
@@ -351,6 +363,41 @@ int vkr_copy_tile_columns(const vkr_shading_pass_desc_t& d, void* dst, const voi
 
 extern "C" int vkr_shading_pass_run(vkr_shading_pass_t* pass, const vkr_device_t* device, const void* constants, size_t constants_size, const void* d_gbuffer, void* d_out_rgba32f) {
 	return launch_shading(pass, device, constants, constants_size, d_gbuffer, d_out_rgba32f);
+}
+
+extern "C" int vkr_shading_pass_run_tiles(vkr_shading_pass_t* pass, const vkr_device_t* device, const void* constants, size_t constants_size, const void* d_gbuffer, void* d_out_rgba32f,
+	const uint32_t* tiles, uint32_t tile_count)
+{
+	if (!tile_count) return 0;
+	const vkr_shading_pass_desc_t& d = pass->desc;
+	const uint32_t frame_tiles = ((d.width + VKR_TILE_WIDTH - 1) / VKR_TILE_WIDTH) * ((d.height + VKR_TILE_ROW_HEIGHT - 1) / VKR_TILE_ROW_HEIGHT);
+	if (!tiles || !pass->h_tile_list) { printf("Failed to shade a tile list: no list, or the shading pass has not been created.\n"); return 1; }
+	if (tile_count > pass->tile_count) { printf("Failed to shade a tile list: %u tiles, but this instance shades %u.\n", tile_count, pass->tile_count); return 1; }
+	std::vector<uint8_t> mark(frame_tiles, 0);   // 1: a tile of this instance, 2: listed already
+	for (uint32_t k = 0; k != pass->tile_count; ++k) mark[((const uint32_t*) pass->h_tile_list)[k]] = 1;
+	for (uint32_t k = 0; k != tile_count; ++k) {
+		const uint32_t t = tiles[k];
+		if (t >= frame_tiles || mark[t] != 1) {
+			printf("Failed to shade a tile list: tile %u (entry %u) is %s.\n", t, k, t >= frame_tiles ? "out of range" : mark[t] ? "listed twice" : "not in this instance's share");
+			return 1;
+		}
+		mark[t] = 2;
+	}
+	if (!pass->d_subset_tiles) {
+		cudaEvent_t e = nullptr;
+		VKR_CUDA_OK(cudaSetDevice(device->cuda_device), "Failed to select the CUDA device");
+		if (cudaMalloc(&pass->d_subset_tiles, sizeof(uint32_t) * pass->tile_count) != cudaSuccess || cudaMallocHost(&pass->h_subset_tiles, sizeof(uint32_t) * pass->tile_count) != cudaSuccess
+			|| cudaEventCreateWithFlags(&e, cudaEventDisableTiming) != cudaSuccess)
+		{
+			printf("Failed to allocate the tile list of the shading pass.\n");
+			if (pass->d_subset_tiles) cudaFree(pass->d_subset_tiles);
+			if (pass->h_subset_tiles) cudaFreeHost(pass->h_subset_tiles);
+			pass->d_subset_tiles = pass->h_subset_tiles = nullptr;
+			return 1;
+		}
+		pass->event_subset = e;
+	}
+	return vkr_launch_shading(pass, device, constants, constants_size, d_gbuffer, d_out_rgba32f, nullptr, 0, nullptr, tiles, tile_count);
 }
 
 extern "C" int vkr_shading_pass_run_with_counters(vkr_shading_pass_t* pass, const vkr_device_t* device, const void* constants, size_t constants_size, const void* d_gbuffer, void* d_out_rgba32f, uint64_t* out_counters) {

@@ -20,7 +20,7 @@
 #define VKR_CUDA_OK(call, what) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { printf("%s: %s\n", what, cudaGetErrorString(e_)); return 1; } } while (0)
 
 int vkr_launch_shading(vkr_shading_pass_t* pass, const vkr_device_t* device, const void* constants, size_t constants_size, const void* d_gbuffer, void* d_out, unsigned long long* d_stats,
-	int peer_count, void* const* peer_outs);   // vkr_api.cu
+	int peer_count, void* const* peer_outs, const uint32_t* subset, uint32_t subset_count);   // vkr_api.cu
 int vkr_copy_tile_columns(const vkr_shading_pass_desc_t& d, void* dst, const void* src, size_t texel, cudaMemcpyKind kind, cudaStream_t stream);   // vkr_api.cu
 extern "C" int vkr_frame_exchange_wait(vkr_frame_exchange_t* e, const vkr_device_t* device);
 
@@ -160,7 +160,7 @@ extern "C" int vkr_shading_pass_run_exchange(vkr_shading_pass_t* pass, const vkr
 		counters.p[r] = counters_of(e, e->d_peer_blocks[r]);
 		if (r != e->rank) peers[peer_count++] = (char*) e->d_peer_blocks[r] + buffer;
 	}
-	if (vkr_launch_shading(pass, device, constants, constants_size, d_gbuffer, (char*) e->d_block + buffer, nullptr, peer_count, peers)) return 1;
+	if (vkr_launch_shading(pass, device, constants, constants_size, d_gbuffer, (char*) e->d_block + buffer, nullptr, peer_count, peers, nullptr, 0)) return 1;
 	if (e->world > 1) {
 		exchange_signal_kernel<<<1, 32, 0, stream>>>(counters, (int) e->world, (int) e->rank, (unsigned long long) frame);
 		int* d_status = nullptr;

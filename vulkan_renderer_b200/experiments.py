@@ -19,6 +19,7 @@ Everything that computes goes through libvkr_b200.so; there is no CPU fallback.
 import ctypes as C
 import json
 import os
+import time
 
 from . import api, synth
 
@@ -262,13 +263,15 @@ def convergence_groups():
 	]
 
 
-def run_convergence(group, data_root, out_dir, reference_frames, variance_frames, width=None, height=None, cuda_device=0, ltc_dir=None, noise_root=None):
+def run_convergence(group, data_root, out_dir, reference_frames, variance_frames, width=None, height=None, cuda_device=0, ltc_dir=None, noise_root=None, adaptive=None):
 	"""Measures the members of one convergence group (convergence_groups()) against a converged reference: the reference experiment's settings
 	averaged over `reference_frames` animated frames. Per member: its screenshot frame (animate_noise = 0, the frame run_experiment shades, in linear
 	radiance) against that reference, and the mean per-frame variance over `variance_frames` animated frames. The record also holds the error of the
 	reference experiment's own screenshot frame (reference_frame_error). With out_dir, the reference is stored as out_dir/convergence/<group>_reference.hdr.
 	ltc_dir: LTC table for the reference and the members instead of the synthetic one; noise_root: Ahmed-Wonka table for the reference and the
-	members instead of white noise (prepare_data). Returns the JSON record."""
+	members instead of white noise (prepare_data). adaptive: a target relMSE; the reference is then built by convergence.accumulate_adaptive with
+	max_frames = reference_frames, and the record's "adaptive" entry says what it shaded, what it cost and its estimated relMSE (its
+	reference_mean_variance is None: the pixels average different frame counts). Returns the JSON record."""
 	from . import convergence
 	by_name = {e["name"]: e for e in experiment_list(all_timings=False)}
 
@@ -281,7 +284,12 @@ def run_convergence(group, data_root, out_dir, reference_frames, variance_frames
 	w = width or ref_experiment["width"]; h = height or ref_experiment["height"]
 	frame = open_frame(ref_experiment)
 	try:
-		reference = convergence.accumulate(frame, w, h, reference_frames, animate=True)
+		if adaptive is None:
+			reference = convergence.accumulate(frame, w, h, reference_frames, animate=True)
+		else:
+			start = time.perf_counter()
+			reference = convergence.accumulate_adaptive(frame, w, h, reference_frames, adaptive)
+			wall_s = time.perf_counter() - start
 		# the reference experiment's own screenshot frame against the converged image: the error of one frame of these settings (for the bias test: unbiased)
 		reference_frame_error = convergence.frame_error(frame, convergence.accumulate(frame, w, h, 1, animate=False).mean, reference.mean)
 		if out_dir is not None:
@@ -293,9 +301,16 @@ def run_convergence(group, data_root, out_dir, reference_frames, variance_frames
 		frame.close()
 	record = dict(group=group["name"], reference=group["reference"], width=w, height=h, ltc=ltc_dir or "synthetic", reference_frames=reference_frames,
 		reference_samples_per_pixel=ref_experiment["settings"]["sample_count"] * reference_frames,
-		reference_mean_variance=list(reference.mean_variance) if reference.mean_variance is not None else None,
-		reference_frame_error=reference_frame_error, accumulate_ms_per_frame=round(reference.accumulate_ms_per_frame, 5), variance_frames=variance_frames,
-		timed="accumulate kernel per frame at %dx%d, CUDA events" % (w, h), members=[])
+		reference_mean_variance=list(reference.mean_variance) if adaptive is None and reference.mean_variance is not None else None,
+		reference_frame_error=reference_frame_error, accumulate_ms_per_frame=round(reference.accumulate_ms_per_frame if adaptive is None else reference.accumulate_ms / reference.frames, 5),
+		variance_frames=variance_frames, timed="accumulate kernel per frame at %dx%d, CUDA events" % (w, h), members=[])
+	if adaptive is not None:
+		record["adaptive"] = dict(target_rel_mse=adaptive, frames=reference.frames, estimated_rel_mse=list(reference.estimated_rel_mse),
+			tile_frames_shaded=reference.tile_frames_shaded, tile_frames_full=reference.tile_frames_full,
+			shaded_fraction=round(reference.tile_frames_shaded / reference.tile_frames_full, 5),
+			tile_frames_min=int(reference.tile_frames.min()), tile_frames_max=int(reference.tile_frames.max()),
+			shade_ms=round(reference.shade_ms, 3), accumulate_ms=round(reference.accumulate_ms, 3), wall_s=round(wall_s, 3),
+			timed="shading and accumulate launches of the reference, CUDA events; wall_s: the whole adaptive reference, host clock")
 	if noise_root is not None:
 		record["noise_root"] = noise_root
 	for name in group["members"]:
@@ -322,6 +337,10 @@ def run_convergences(groups, data_root, out_dir, json_path, reference_frames, va
 		records.append(record)
 		print("%s against %s (%d frames, %dx%d; accumulate %.4f ms per frame)" % (group["name"], group["reference"], reference_frames, record["width"], record["height"],
 			record["accumulate_ms_per_frame"]), flush=True)
+		if "adaptive" in record:
+			a = record["adaptive"]
+			print("  adaptive reference, target relMSE %g: %d of %d tile-frames shaded (%.3f), estimated relMSE %.4e, shading %.1f ms, %.2f s" % (a["target_rel_mse"],
+				a["tile_frames_shaded"], a["tile_frames_full"], a["shaded_fraction"], sum(a["estimated_rel_mse"]) / 3.0, a["shade_ms"], a["wall_s"]), flush=True)
 		e = record["reference_frame_error"]
 		print("  %-70s relMSE %.4e  MSE %.4e" % ("(one frame of the reference's settings)", sum(e["rel_mse"]) / 3.0, sum(e["mse"]) / 3.0), flush=True)
 		for m in sorted(record["members"], key=lambda m: sum(m["rel_mse"])):
