@@ -511,6 +511,22 @@ int vkr_write_hdr(const char* file_path, uint32_t width, uint32_t height, const 
    constants: HOST pointer; d_gbuffer: DEVICE pointer. Synchronous. */
 int vkr_take_screenshot(vkr_shading_pass_t* pass, const vkr_device_t* device, const void* constants, size_t constants_size, const void* d_gbuffer,
 	const char* path_png, const char* path_hdr);
+/* The reference's three-path take_screenshot (src/main.c:1550-1566): any of *.png, *.jpg and *.hdr may be NULL; LDR (png, jpg) and HDR cannot be
+   mixed, png and jpg are written from the same frame. The *.jpg is quantised (vkr_quantize_unorm8_device) and encoded on the device at quality 70
+   (stbi_write_jpg at src/main.c:1745-1751); *.png and *.hdr are written as vkr_take_screenshot writes them, which calls this with path_jpg = NULL. */
+int vkr_take_screenshot_formats(vkr_shading_pass_t* pass, const vkr_device_t* device, const void* constants, size_t constants_size, const void* d_gbuffer,
+	const char* path_png, const char* path_jpg, const char* path_hdr);
+/* vkr_quantize_unorm8 on the device, bit for bit: DEVICE float4 frame (width*height, 16-byte aligned) -> DEVICE tightly packed RGB bytes.
+   Asynchronous on device->stream. */
+int vkr_quantize_unorm8_device(const vkr_device_t* device, const void* d_rgba32f, uint32_t width, uint32_t height, void* d_rgb8);
+/* ---- JPEG files (csrc/vkr_jpeg.cu; DESIGN.md §5): baseline JPEG, byte-identical to stbi_write_jpg (stb_image_write v1.14) for the same 8-bit RGB image
+        and quality. quality 0 means 90, anything else is clamped to 1..100; quality <= 90 subsamples chroma 4:2:0, above it 4:4:4. Sizes 1..65535
+        per side (SOF0's 16 bits). Encoded on the device (device->stream); synchronous. */
+/* d_rgb8: DEVICE image, width*height*3 bytes as vkr_quantize_unorm8 lays them out. The file goes to out_file and *out_size is its size. If the file
+   is larger than capacity, returns 1 with nothing written and *out_size = the size needed. Refuses NULL pointers and sizes outside 1..65535. */
+int vkr_encode_jpg(const vkr_device_t* device, const uint8_t* d_rgb8, uint32_t width, uint32_t height, int quality, uint8_t* out_file, size_t capacity, size_t* out_size);
+/* rgb8: HOST image (the counterpart of vkr_write_png), encoded on the device and stored at path */
+int vkr_write_jpg(const vkr_device_t* device, const char* path, uint32_t width, uint32_t height, const uint8_t* rgb8, int quality);
 /* record_frame_time / get_frame_time, src/frame_timer.c:28-75: median of the differences of the last 100 recorded times (seconds) */
 void vkr_record_frame_time(double time_in_seconds);
 float vkr_get_frame_time(void);

@@ -32,6 +32,7 @@ EXPORTED_SYMBOLS = [
 	"vkr_adaptive_tile_frames", "vkr_adaptive_resolve", "vkr_adaptive_estimated_rel_mse",
 	"vkr_ltc_fit_default_desc", "vkr_fit_ltc_table", "vkr_write_ltc_fits",
 	"vkr_noise_gen_default_desc", "vkr_generate_noise_table", "vkr_write_noise_table",
+	"vkr_take_screenshot_formats", "vkr_quantize_unorm8_device", "vkr_encode_jpg", "vkr_write_jpg",
 ]
 
 # enums (values = the reference's)
@@ -266,6 +267,10 @@ def load_library():
 	lib.vkr_write_png.argtypes = [C.c_char_p, C.c_uint32, C.c_uint32, C.c_void_p]
 	lib.vkr_write_hdr.argtypes = [C.c_char_p, C.c_uint32, C.c_uint32, C.c_void_p]
 	lib.vkr_take_screenshot.argtypes = [P(ShadingPass), P(Device), C.c_void_p, C.c_size_t, C.c_void_p, C.c_char_p, C.c_char_p]
+	lib.vkr_take_screenshot_formats.argtypes = [P(ShadingPass), P(Device), C.c_void_p, C.c_size_t, C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p]
+	lib.vkr_quantize_unorm8_device.argtypes = [P(Device), C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p]
+	lib.vkr_encode_jpg.argtypes = [P(Device), C.c_void_p, C.c_uint32, C.c_uint32, C.c_int, C.c_void_p, C.c_size_t, P(C.c_size_t)]
+	lib.vkr_write_jpg.argtypes = [P(Device), C.c_char_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_int]
 	lib.vkr_record_frame_time.argtypes = [C.c_double]; lib.vkr_record_frame_time.restype = None
 	lib.vkr_get_frame_time.argtypes = []; lib.vkr_get_frame_time.restype = C.c_float
 	lib.vkr_reset_frame_times.argtypes = []; lib.vkr_reset_frame_times.restype = None

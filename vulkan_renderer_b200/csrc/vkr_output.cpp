@@ -8,6 +8,7 @@
 // Host code: no contraction (-ffp-contract=off).
 #include "vkr_b200.h"
 #include "vkr_internal.h"
+#include "vkr_jpeg.cuh"
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdio.h>
@@ -72,9 +73,7 @@ extern "C" void vkr_quantize_unorm8(const float* rgba32f, uint32_t width, uint32
 	const size_t pixel_count = (size_t) width * height;
 	for (size_t i = 0; i != pixel_count; ++i)
 		for (int c = 0; c != 3; ++c) {
-			float x = rgba32f[4 * i + c];
-			x = (x > 0.0f) ? ((x < 1.0f) ? x : 1.0f) : 0.0f;
-			out_rgb8[3 * i + c] = (uint8_t) (x * 255.0f + 0.5f);
+			out_rgb8[3 * i + c] = vkr_jpeg::unorm8(rgba32f[4 * i + c]);   // the device quantisation of JPEG screenshots shares it
 		}
 }
 
@@ -237,42 +236,67 @@ extern "C" float vkr_get_frame_time(void) {
 // Screenshot of one frame (take_screenshot + implement_screenshot, src/main.c:1550-1770). LDR: the shader converts to sRGB, the
 // 8-bit target quantises. HDR: two LDR frames carry the low and the high bytes of the half-precision colours (g_frame_bits = 1, 2;
 // shading_pass.frag.glsl:871-887) and are combined on the host -- kept as the reference does it so that the files agree.
-extern "C" int vkr_take_screenshot(vkr_shading_pass_t* pass, const vkr_device_t* device, const void* constants, size_t constants_size, const void* d_gbuffer,
-	const char* path_png, const char* path_hdr)
+// *.jpg (stbi_write_jpg at quality 70, src/main.c:1745-1751): the frame is quantised and encoded on the device (vkr_jpeg.cu), so only the
+// file comes back.
+static const int kScreenshotJpegQuality = 70;
+
+extern "C" int vkr_take_screenshot_formats(vkr_shading_pass_t* pass, const vkr_device_t* device, const void* constants, size_t constants_size, const void* d_gbuffer,
+	const char* path_png, const char* path_jpg, const char* path_hdr)
 {
-	if (path_png && path_hdr) { printf("Cannot mix LDR and HDR screenshots.\n"); return 1; }
-	if (!path_png && !path_hdr) return 0;
+	if ((path_png || path_jpg) && path_hdr) { printf("Cannot mix LDR and HDR screenshots.\n"); return 1; }
+	if (!path_png && !path_jpg && !path_hdr) return 0;
 	const uint32_t width = pass->desc.width, height = pass->desc.height;
 	const size_t pixel_count = (size_t) width * height;
 	if (constants_size != pass->constants_size || pass->desc.stripe_count > 1) { printf("Failed to take a screenshot: wrong constant block size or a striped pass.\n"); return 1; }
+	const bool host_frame = path_png || path_hdr;   // *.png and *.hdr are written from the frame on the host
 	std::vector<uint8_t> block((const uint8_t*) constants, (const uint8_t*) constants + constants_size);
-	std::vector<float> frame(4 * pixel_count);
-	std::vector<uint8_t> ldr(3 * pixel_count * (path_hdr ? 2 : 1));
+	std::vector<float> frame(host_frame ? 4 * pixel_count : 0);
+	std::vector<uint8_t> ldr(host_frame ? 3 * pixel_count * (path_hdr ? 2 : 1) : 0);
 	void* d_frame = nullptr;
-	if (cudaSetDevice(device->cuda_device) != cudaSuccess || cudaMalloc(&d_frame, sizeof(float) * 4 * pixel_count) != cudaSuccess) {
-		printf("Failed to create a staging image for taking a screenshot.\n"); return 1;
+	void* d_rgb8 = nullptr;
+	if (cudaSetDevice(device->cuda_device) != cudaSuccess || cudaMalloc(&d_frame, sizeof(float) * 4 * pixel_count) != cudaSuccess
+		|| (path_jpg && cudaMalloc(&d_rgb8, 3 * pixel_count) != cudaSuccess))
+	{
+		printf("Failed to create a staging image for taking a screenshot.\n");
+		if (d_frame) cudaFree(d_frame);
+		return 1;
 	}
 	const int saved_srgb = pass->desc.output_srgb;
 	pass->desc.output_srgb = 1; // an UNORM render target: the shader itself converts to sRGB (OUTPUT_LINEAR_RGB=0)
 	int failed = 0;
 	for (uint32_t frame_bits = (path_hdr ? 1u : 0u); frame_bits <= (path_hdr ? 2u : 0u) && !failed; ++frame_bits) {
 		vkr_set_frame_bits(block.data(), frame_bits);
-		failed = vkr_shading_pass_run(pass, device, block.data(), constants_size, d_gbuffer, d_frame) || vkr_shading_pass_wait(pass, device)
-			|| cudaMemcpy(frame.data(), d_frame, sizeof(float) * 4 * pixel_count, cudaMemcpyDeviceToHost) != cudaSuccess;
-		if (!failed) vkr_quantize_unorm8(frame.data(), width, height, ldr.data() + (frame_bits == 2 ? 3 * pixel_count : 0));
+		failed = vkr_shading_pass_run(pass, device, block.data(), constants_size, d_gbuffer, d_frame) || vkr_shading_pass_wait(pass, device);
+		if (!failed && path_jpg) failed = vkr::jpeg_quantize(device, (const float*) d_frame, width, height, (uint8_t*) d_rgb8);
+		if (!failed && host_frame) {
+			failed = cudaMemcpy(frame.data(), d_frame, sizeof(float) * 4 * pixel_count, cudaMemcpyDeviceToHost) != cudaSuccess;
+			if (!failed) vkr_quantize_unorm8(frame.data(), width, height, ldr.data() + (frame_bits == 2 ? 3 * pixel_count : 0));
+		}
 	}
 	pass->desc.output_srgb = saved_srgb;
+	if (failed) printf("Failed to render the frame for a screenshot.\n");
+	else if (path_jpg) {
+		failed = vkr::jpeg_write_device_image(device, path_jpg, (const uint8_t*) d_rgb8, width, height, kScreenshotJpegQuality);
+		if (!failed) printf("Wrote screenshot to %s.\n", path_jpg);
+	}
 	cudaFree(d_frame);
-	if (failed) { printf("Failed to render the frame for a screenshot.\n"); return 1; }
+	if (d_rgb8) cudaFree(d_rgb8);
+	if (failed) return 1;
 	if (path_png) {
 		if (vkr_write_png(path_png, width, height, ldr.data())) return 1;
 		printf("Wrote screenshot to %s.\n", path_png);
 	}
-	else {
+	else if (path_hdr) {
 		std::vector<float> hdr(3 * pixel_count);
 		vkr_combine_ldr_screenshots_into_hdr(ldr.data(), ldr.data() + 3 * pixel_count, 3 * pixel_count, hdr.data());
 		if (vkr_write_hdr(path_hdr, width, height, hdr.data())) return 1;
 		printf("Wrote screenshot to %s.\n", path_hdr);
 	}
 	return 0;
+}
+
+extern "C" int vkr_take_screenshot(vkr_shading_pass_t* pass, const vkr_device_t* device, const void* constants, size_t constants_size, const void* d_gbuffer,
+	const char* path_png, const char* path_hdr)
+{
+	return vkr_take_screenshot_formats(pass, device, constants, constants_size, d_gbuffer, path_png, nullptr, path_hdr);
 }
