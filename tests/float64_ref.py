@@ -1,5 +1,7 @@
-"""Plain float64 references for the two primitives every frame rests on: projected-solid-angle (PSA) sampling of a horizon-clipped polygon
-(vkr_psa.cuh) and the any-hit shadow query (vkr_trace.cuh). numpy only; nothing here shares code or operation order with the oracle or the kernels.
+"""Plain float64 references for the two primitives every frame rests on, projected-solid-angle (PSA) sampling of a horizon-clipped polygon
+(vkr_psa.cuh) and the any-hit shadow query (vkr_trace.cuh), and for what a frame estimates: the BRDF (brdfs.glsl) and the direct lighting, the
+BRDF times the cosine integrated over the lights minus what occluders cover (direct_lighting). numpy only; nothing here shares code or operation
+order with the oracle or the kernels.
 
 Polygons are (n, 3) arrays of vertices seen from the origin, the shading normal is +z. Rays are rows {ox, oy, oz, dx, dy, dz, tmin, tmax}.
 """
@@ -166,3 +168,136 @@ def shadow_truth(tris, rays, rel_margin=2.0 ** -20, chunk_elements=1 << 21):
 			hit[s:s + step] = any_hit
 			decided[s:s + step] = any_hit | clear_miss.all(axis=1) | empty
 	return hit, decided
+
+
+# ---- the shading pass's integral: BRDF times cosine times radiance over the lights, with occluders ------------------------------------------
+
+def brdf(wi, wo, n, albedo, f0, roughness):
+	"""The BRDF of brdfs.glsl (diffuse and specular lobes, each on or off), in world space, for unit incoming directions wi [m, 3] and one unit
+	outgoing direction wo and normal n: Frostbite's diffuse term albedo / pi * F_D(n.wo) * F_D(n.wi) with F_D(c) = 1 + (F90 - 1) (1 - c)^5,
+	F90 = 0.5 + 2 roughness (wo.h)^2, plus GGX with alpha = roughness, height-correlated Smith and Schlick's Fresnel per channel of f0
+	(ltc_fit.specular_brdf). Returns (diffuse [m, 3], specular [m, 3])."""
+	from vulkan_renderer_b200.ltc_fit import specular_brdf
+	wi = np.asarray(wi, dtype=np.float64); wo = np.asarray(wo, dtype=np.float64); n = np.asarray(n, dtype=np.float64)
+	t, b = _tangent_frame(n)
+	local = np.stack([wi @ t, wi @ b, wi @ n], axis=-1)
+	wo_local = np.array([wo @ t, wo @ b, wo @ n])
+	h = local + wo_local
+	h /= np.linalg.norm(h, axis=-1, keepdims=True)
+	oh = h @ wo_local
+	f90 = 0.5 + 2.0 * roughness * oh * oh
+	schlick = lambda c: 1.0 + (f90 - 1.0) * (1.0 - c) ** 5
+	diffuse = (schlick(wo_local[2]) * schlick(local[:, 2]))[:, None] * np.asarray(albedo, dtype=np.float64)[None] / math.pi
+	specular = np.stack([specular_brdf(wo_local, local, roughness, float(f)) for f in f0], axis=-1)
+	return diffuse, specular
+
+
+def _tangent_frame(n):
+	n = np.asarray(n, dtype=np.float64)
+	a = np.array([1.0, 0.0, 0.0]) if abs(n[0]) < 0.8 else np.array([0.0, 1.0, 0.0])
+	t = a - (a @ n) * n; t /= np.linalg.norm(t)
+	return t, np.cross(n, t)
+
+
+_GAUSS_NODES, _GAUSS_WEIGHTS = np.polynomial.legendre.leggauss(8)
+_GAUSS_NODES = 0.5 * (_GAUSS_NODES + 1.0); _GAUSS_WEIGHTS = 0.5 * _GAUSS_WEIGHTS
+
+
+def _triangle_rule(tris, g):
+	"""Gauss-Legendre 8 x 8 through the Duffy map (s, t) -> a + s (b - a) + s t (c - b), Jacobian 2 area s, for triangles [T, 3, 3]: [T, c]."""
+	s = _GAUSS_NODES[:, None]; t = _GAUSS_NODES[None, :]
+	a, b, c = tris[:, 0], tris[:, 1], tris[:, 2]
+	p = a[:, None, None] + s[None, :, :, None] * (b - a)[:, None, None] + (s * t)[None, :, :, None] * (c - b)[:, None, None]
+	w = (_GAUSS_WEIGHTS[:, None] * _GAUSS_WEIGHTS[None, :] * s)[None] * np.linalg.norm(np.cross(b - a, c - b), axis=-1)[:, None, None]
+	values = g(p.reshape(-1, 3)).reshape(len(tris), len(_GAUSS_NODES), len(_GAUSS_NODES), -1)
+	return (values * w[..., None]).sum(axis=(1, 2))
+
+
+def integrate_polygon(poly, g, rtol=1e-10, atol=0.0, max_levels=40, max_triangles=1 << 16):
+	"""The integral of g (points [m, 3] -> values [m, c]) over a planar convex polygon [k, 3]: a fan of triangles, each refined 4 ways (midpoints of
+	the edges) until the rule on a triangle and the sum of the rule on its four children agree to rtol of the whole (or to atol, if larger), with
+	each triangle's share of the tolerance in proportion to its area. Returns (integral [c], levels used)."""
+	P = np.asarray(poly, dtype=np.float64)
+	tris = np.stack([np.broadcast_to(P[0], (len(P) - 2, 3)), P[1:-1], P[2:]], axis=1)
+	area_of = lambda T: 0.5 * np.linalg.norm(np.cross(T[:, 1] - T[:, 0], T[:, 2] - T[:, 0]), axis=-1)
+	total_area = float(area_of(tris).sum())
+	if total_area == 0.0:
+		return 0.0, 0
+	parent = _triangle_rule(tris, g)
+	result = np.zeros(parent.shape[1])
+	scale = None
+	for level in range(max_levels):
+		m = (tris + np.roll(tris, -1, axis=1)) * 0.5      # midpoints of the edges ab, bc, ca
+		kids = np.stack([np.stack([tris[:, 0], m[:, 0], m[:, 2]], 1), np.stack([m[:, 0], tris[:, 1], m[:, 1]], 1),
+			np.stack([m[:, 2], m[:, 1], tris[:, 2]], 1), np.stack([m[:, 0], m[:, 1], m[:, 2]], 1)], axis=1)
+		child = _triangle_rule(kids.reshape(-1, 3, 3), g).reshape(len(tris), 4, -1)
+		fine = child.sum(axis=1)
+		if scale is None:
+			scale = max(float(np.abs(fine.sum(axis=0)).max()), atol / rtol, 1e-300)
+		done = np.abs(fine - parent).max(axis=1) <= rtol * scale * area_of(tris) / total_area
+		result += fine[done].sum(axis=0)
+		if done.all():
+			return result, level + 1
+		tris = kids[~done].reshape(-1, 3, 3); parent = child[~done].reshape(-1, child.shape[2])
+		if len(tris) > max_triangles:
+			break
+	raise RuntimeError("integrate_polygon: no convergence to %g after %d levels, %d triangles left" % (rtol, level + 1, len(tris)))
+
+
+def _plane_normal(poly):
+	P = np.asarray(poly, dtype=np.float64)
+	nrm = sum(np.cross(P[i] - P[0], P[i + 1] - P[0]) for i in range(1, len(P) - 1))
+	return nrm / np.linalg.norm(nrm)
+
+
+def light_integral(x, n, poly, g, occluders=(), planes=(), rtol=1e-10):
+	"""The integral over directions w of g(w) [m, c] where the light polygon [k, 3] (world space, emitting on both faces) lies above x's tangent
+	plane (n . w > 0) and on the positive side of the extra planes through x (normals `planes`), minus the part whose segment to x crosses one of
+	the occluder triangles [3, 3]. Integrated over the polygon's area with dw = |n_L . (p - x)| / |p - x|^3 dA. Each occluder must lie strictly
+	between x and the light's plane, their central projections onto it must not overlap (the two halves of a quad do not)."""
+	x = np.asarray(x, dtype=np.float64); n = np.asarray(n, dtype=np.float64)
+	P = np.asarray(poly, dtype=np.float64) - x
+	nl = _plane_normal(P); height = float(P[0] @ nl)
+	def integrand(p):
+		r = np.linalg.norm(p, axis=-1)
+		return g(p / r[:, None]) * (abs(height) / r ** 3)[:, None]
+	def region_integral(region, atol=0.0):
+		return integrate_polygon(np.array(region), integrand, rtol, atol)[0] if len(region) >= 3 else 0.0
+	region = _clip_halfspace([tuple(p) for p in P], tuple(n))
+	atol = 0.0
+	if len(planes):   # a sliver cut off by the extra planes is integrated to rtol of the whole light, not of itself
+		atol = rtol * float(np.abs(region_integral(region)).max())
+	for normal in planes:
+		region = _clip_halfspace(region, tuple(normal)) if len(region) >= 3 else region
+	total = unshadowed = region_integral(region, atol)
+	for tri in occluders:
+		T = np.asarray(tri, dtype=np.float64) - x
+		depth = (T @ nl) / height                        # 0 at x, 1 on the light's plane
+		if (depth <= 0.0).all() or (depth >= 1.0).all():
+			continue
+		if not ((depth > 0.0) & (depth < 1.0)).all():
+			raise ValueError("an occluder crosses x's plane or the light's plane: %s" % tri)
+		shadow = region
+		centre = T.mean(axis=0)
+		for i in range(3):
+			e = np.cross(T[i], T[(i + 1) % 3])
+			e = e if e @ centre > 0.0 else -e
+			shadow = _clip_halfspace(shadow, tuple(e)) if len(shadow) >= 3 else shadow
+		total = total - region_integral(shadow, atol)
+	# a fully shadowed light leaves the quadrature's rounding, not light
+	return np.where(np.abs(total) <= 10.0 * rtol * np.abs(unshadowed), 0.0, np.atleast_1d(total))
+
+
+def direct_lighting(x, n, wo, albedo, f0, roughness, lights, occluders=(), lobes=(True, True), planes=(), rtol=1e-10):
+	"""Sum over lights (vertices [k, 3], radiance [3]) of L_e times the integral of f(w) (n . w) over the visible part of the light above x's
+	tangent plane: the outgoing radiance the shading pass estimates, in float64. lobes: (diffuse, specular) of the BRDF; planes, occluders: see
+	light_integral. Returns [3]."""
+	n = np.asarray(n, dtype=np.float64)
+	def g(w):
+		diffuse, specular = brdf(w, wo, n, albedo, f0, roughness)
+		f = (diffuse if lobes[0] else 0.0) + (specular if lobes[1] else 0.0)
+		return f * np.maximum(w @ n, 0.0)[:, None]
+	total = np.zeros(3)
+	for poly, radiance in lights:
+		total += np.asarray(radiance, dtype=np.float64) * light_integral(x, n, poly, g, occluders, planes, rtol)
+	return total
