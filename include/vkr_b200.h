@@ -341,9 +341,32 @@ size_t vkr_gbuffer_size(uint32_t width, uint32_t height);
 int vkr_run_visibility_pass(const vkr_device_t* device, const vkr_scene_t* scene, const void* constants, uint32_t width, uint32_t height, void* d_visibility);
 int vkr_run_gbuffer_pass(const vkr_device_t* device, const vkr_scene_t* scene, const void* constants, uint32_t width, uint32_t height, const void* d_visibility, void* d_gbuffer);
 
+/* ---- rasterised visibility: subpass 0 of the reference (src/main.c:1421-1427, visibility_pass.{vert,frag}.glsl) with its fixed-function state:
+        back faces culled (frontFace = COUNTER_CLOCKWISE), clipping to 0 <= z <= w, one sample at the pixel centre, depth test LESS against a
+        D32_SFLOAT buffer cleared to 1.0 in draw order. Vulkan leaves sub-pixel precision and depth arithmetic open; DESIGN.md §5 "Rasterised
+        visibility" fixes them (8 sub-pixel bits, fp64 depth rounded once to binary32). Unlike vkr_run_visibility_pass it culls and clips, so the
+        two buffers differ; it needs no acceleration structure. The rasterizer owns the depth-test keys and the per-triangle scratch, so a call
+        allocates nothing. At most 32768 pixels per side. */
+typedef struct vkr_rasterizer_s {
+	uint32_t width, height;
+	uint64_t triangle_capacity;   /* the largest scene it can draw */
+	void* d_keys;                 /* uint64 per pixel: depth bits << 32 | primitive index */
+	void* d_scratch;              /* per triangle: chunks of its box if it is large and their inclusive scan (8 B each), then the scan's temporary storage */
+	void* d_constants;            /* device copy of the constant block's first 256 bytes */
+	uint64_t scratch_bytes, scan_temp_bytes;
+	uint32_t large_ctas;          /* CTAs of the large-triangle kernel */
+} vkr_rasterizer_t;
+int vkr_create_rasterizer(vkr_rasterizer_t* rasterizer, const vkr_device_t* device, uint32_t width, uint32_t height, uint64_t triangle_capacity);
+void vkr_destroy_rasterizer(vkr_rasterizer_t* rasterizer, const vkr_device_t* device);
+/* d_visibility: uint32 per pixel as vkr_run_visibility_pass writes it (0xFFFFFFFF where nothing was drawn); d_depth: float per pixel, 1.0 where
+   nothing was drawn, may be NULL. constants = first 256 bytes of the block (host). Asynchronous on device->stream. Returns non-zero and launches
+   nothing on NULL arguments, a rasterizer that was not created, a scene larger than triangle_capacity or without positions on the device. */
+int vkr_rasterize_visibility(vkr_rasterizer_t* rasterizer, const vkr_device_t* device, const vkr_scene_t* scene, const void* constants, void* d_visibility, void* d_depth);
+
 /* ---- render targets (replaces create_render_targets / destroy_render_targets, src/main.c:253-315, and the swapchain image the
         shading pass writes): device images of one resolution, owned by the library so that a host application needs no CUDA
-        allocator of its own. The reference's depth buffer has no counterpart (visibility comes from primary rays). */
+        allocator of its own. The reference's depth buffer is not among them: vkr_rasterize_visibility writes it into a caller's buffer (d_depth) when
+        asked for. */
 typedef struct vkr_render_targets_s {
 	uint32_t width, height;
 	void* d_visibility;   /* uint32 per pixel, 0xFFFFFFFF = background (the clear value, src/main.c:1409) */

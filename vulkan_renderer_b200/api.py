@@ -33,6 +33,7 @@ EXPORTED_SYMBOLS = [
 	"vkr_ltc_fit_default_desc", "vkr_fit_ltc_table", "vkr_write_ltc_fits",
 	"vkr_noise_gen_default_desc", "vkr_generate_noise_table", "vkr_write_noise_table",
 	"vkr_take_screenshot_formats", "vkr_quantize_unorm8_device", "vkr_encode_jpg", "vkr_write_jpg",
+	"vkr_create_rasterizer", "vkr_destroy_rasterizer", "vkr_rasterize_visibility",
 ]
 
 # enums (values = the reference's)
@@ -147,6 +148,12 @@ class FrameExchange(C.Structure):
 class Accumulator(C.Structure):
 	"""vkr_accumulator_t: running mean and sum of squared deviations of frames, float64 (include/vkr_b200.h)."""
 	_fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("frame_count", C.c_uint64), ("d_state", C.c_void_p), ("d_partials", C.c_void_p), ("h_partials", C.c_void_p)]
+
+
+class Rasterizer(C.Structure):
+	"""vkr_rasterizer_t: the rasterised visibility buffer (DESIGN.md §5 "Rasterised visibility")"""
+	_fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("triangle_capacity", C.c_uint64), ("d_keys", C.c_void_p), ("d_scratch", C.c_void_p),
+		("d_constants", C.c_void_p), ("scratch_bytes", C.c_uint64), ("scan_temp_bytes", C.c_uint64), ("large_ctas", C.c_uint32)]
 
 
 class AdaptiveAccumulator(C.Structure):
@@ -274,6 +281,9 @@ def load_library():
 	lib.vkr_record_frame_time.argtypes = [C.c_double]; lib.vkr_record_frame_time.restype = None
 	lib.vkr_get_frame_time.argtypes = []; lib.vkr_get_frame_time.restype = C.c_float
 	lib.vkr_reset_frame_times.argtypes = []; lib.vkr_reset_frame_times.restype = None
+	lib.vkr_create_rasterizer.argtypes = [P(Rasterizer), P(Device), C.c_uint32, C.c_uint32, C.c_uint64]
+	lib.vkr_destroy_rasterizer.argtypes = [P(Rasterizer), P(Device)]; lib.vkr_destroy_rasterizer.restype = None
+	lib.vkr_rasterize_visibility.argtypes = [P(Rasterizer), P(Device), P(Scene), C.c_void_p, C.c_void_p, C.c_void_p]
 	lib.vkr_create_accumulator.argtypes = [P(Accumulator), P(Device), C.c_uint32, C.c_uint32]
 	lib.vkr_destroy_accumulator.argtypes = [P(Accumulator), P(Device)]; lib.vkr_destroy_accumulator.restype = None
 	lib.vkr_accumulator_reset.argtypes = [P(Accumulator), P(Device)]

@@ -118,16 +118,27 @@ class Frame:
 		self._passes = [q for q in self._passes if q is not p]
 
 	# ---- host-buffer conveniences built on cudaMalloc'ed scratch inside the library (tests, smoke)
-	def gbuffer_host(self, width, height):
-		"""Runs the visibility + G-buffer producer on the device and returns (visibility, gbuffer) as numpy arrays."""
+	def gbuffer_host(self, width, height, visibility="ray"):
+		"""Runs the visibility + G-buffer producer on the device and returns (visibility, gbuffer) as numpy arrays. visibility = "ray": the primary-ray
+		cast (vkr_run_visibility_pass, needs the acceleration structure); "raster": the reference's subpass 0, culled and clipped (vkr_rasterize_visibility)."""
 		import torch
+		if visibility not in ("ray", "raster"):
+			raise ValueError("visibility must be 'ray' or 'raster', not %r" % (visibility,))
 		dev = torch.device("cuda", self.device.cuda_device)
 		with torch.cuda.device(dev):
 			vis = torch.empty((height, width), dtype=torch.int32, device=dev)
 			gb = torch.empty((4, height, width, 4), dtype=torch.float32, device=dev)
 			constants = self.constants(width, height)
 			torch.cuda.synchronize()
-			self._check(self.lib.vkr_run_visibility_pass(C.byref(self.device), C.byref(self.scene), constants, width, height, vis.data_ptr()), "vkr_run_visibility_pass")
+			if visibility == "ray":
+				self._check(self.lib.vkr_run_visibility_pass(C.byref(self.device), C.byref(self.scene), constants, width, height, vis.data_ptr()), "vkr_run_visibility_pass")
+			else:
+				r = api.Rasterizer()
+				self._check(self.lib.vkr_create_rasterizer(C.byref(r), C.byref(self.device), width, height, max(self.scene.triangle_count, 1)), "vkr_create_rasterizer")
+				try:
+					self._check(self.lib.vkr_rasterize_visibility(C.byref(r), C.byref(self.device), C.byref(self.scene), constants, vis.data_ptr(), None), "vkr_rasterize_visibility")
+				finally:
+					self.lib.vkr_destroy_rasterizer(C.byref(r), C.byref(self.device))
 			self._check(self.lib.vkr_run_gbuffer_pass(C.byref(self.device), C.byref(self.scene), constants, width, height, vis.data_ptr(), gb.data_ptr()), "vkr_run_gbuffer_pass")
 			self._check(self.lib.vkr_device_wait_idle(C.byref(self.device)), "vkr_device_wait_idle")
 			return vis.cpu().numpy().view(np.uint32), gb.cpu().numpy()
