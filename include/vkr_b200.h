@@ -108,12 +108,12 @@ typedef struct vkr_scene_s {
 	void* d_texture_dims;      /* uint32[4] per texture: width, height, mip_count, 0; order: material-major, {base colour, specular, normal} */
 	void* d_texture_offsets;   /* uint64 per texture: first texel of level 0 in d_texture_data */
 	uint64_t texture_texel_count;
-	uint32_t shadow_bvh_width;  /* children per node of d_shadow_nodes: 2 (64-byte node pairs); 4 only with VKR_BVH_WIDTH=4 in the environment, for the experimental kernel variant */
-	/* the node pairs of d_shadow_nodes once more, 32 bytes each: child boxes as 16-bit coordinates on a grid over the scene, rounded outwards (what the trace
-	   warps of the shading kernels fetch; the float pairs serve the probes and the tests). shadow_grid = minimum xyz, cells per world unit xyz */
+	uint32_t shadow_bvh_width;  /* children per node of d_shadow_nodes: always 2 (64-byte node pairs) */
+	/* unused: always NULL and zero (a quantised copy of the node pairs and its grid, which no kernel reads any more; kept for the layout) */
 	void* d_shadow_nodes_quantised;
 	float shadow_grid[6];
-	/* and once more as interleaved pairs (64 bytes, the two children's numbers side by side: the packed-FMA edition of the trace warps, vkr_trace.cuh) */
+	/* the node pairs of d_shadow_nodes once more, interleaved (64 bytes, the two children's numbers side by side): what the trace warps of the shading
+	   kernels fetch (vkr_trace.cuh); the plain pairs serve the probes and the tests */
 	void* d_shadow_nodes_interleaved;
 } vkr_scene_t;
 

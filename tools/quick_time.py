@@ -4,9 +4,6 @@ import ctypes as C, os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path.insert(0, ROOT)
 import torch
 from vulkan_renderer_b200 import Frame, api, synth
-if os.environ.get("VKR_B200_LIB"):   # tuning variants (tools/build_variant.sh): replace the library the package loaded on import
-	api.LIB_PATH = os.environ["VKR_B200_LIB"]; api._lib = None
-	print("library:", api.LIB_PATH, flush=True)
 spp = int(sys.argv[1]) if len(sys.argv) > 1 else 64
 lights = int(sys.argv[2]) if len(sys.argv) > 2 else 8
 rays = int(sys.argv[3]) if len(sys.argv) > 3 else 1

@@ -9,11 +9,12 @@
 //                 child that continues the chain; the chain is cut after kPathLevels pairs, its end ("tail") is then an inner node.
 //   light cone    per (pixel, light), once: a cone with apex o around the light polygon and the distance of its farthest vertex. A sibling whose
 //                 box (its bounding sphere, to be exact) lies outside the cone cannot be hit by a ray to this light: one bit per path level.
-//   the ray       starts with the tail and the surviving siblings instead of the root (vkr_ray_stream.cuh): a sibling step is an ordinary
+//   the ray       starts with the tail and the surviving siblings instead of the root: a sibling step is an ordinary
 //                 node visit with the chain's child masked out.
 // Soundness does not rest on the sampler: every ray is checked against the cone when it is submitted (ray_in_cone, with the thresholds the
 // cone was built from; the culling uses a slightly wider and longer cone), and a ray that is not inside keeps all siblings. Hit / miss stays
 // the OR over all triangles the predicate accepts, so frames are bit-identical to the plain traversal.
+// No shading kernel starts its rays this way (DESIGN.md section 3, editions of the trace warps that were removed); the CPU tests run these pieces.
 #pragma once
 #include "vkr_trace.cuh"
 
@@ -147,7 +148,7 @@ VKR_DEV int visit_pair(const float4* __restrict__ nodes, int pair, int skip, con
 	return h0 ? ref0 : (h1 ? ref1 : kTraversalDone);
 }
 
-// Per-thread any-hit query of an anchored ray: the reference form of what the trace warps do (vkr_ray_stream.cuh), run on the CPU against occluded() by
+// Per-thread any-hit query of an anchored ray, run on the CPU against occluded() by
 // tests/test_device_on_host.py. path / count / tail: find_origin_path(o); mask: cull_siblings() for a cone the ray is inside of, or kAllSiblings.
 VKR_DEV bool occluded_anchored(const bvh_view& bvh, f3 o, f3 d, float tmin, float tmax, const uint32_t* path, int count, int tail, uint32_t mask, int* stack, int stride, int* visits) {
 	if (!(tmax > tmin)) return false;

@@ -297,11 +297,8 @@ int vkr_launch_shading(vkr_shading_pass_t* pass, const vkr_device_t* device, con
 	if (d.trace_shadow_rays) {
 		p.bvh_nodes = (const float4*) d.scene->d_shadow_nodes; p.bvh_tris = (const float4*) d.scene->d_shadow_tris; p.tri_count = (uint32_t) d.scene->triangle_count;
 		p.stack_depth = (int) d.scene->shadow_max_depth + 2;
-		p.bvh_width = d.scene->shadow_bvh_width ? (int) d.scene->shadow_bvh_width : 2;
-		p.bvh_nodes_q = (const uint4*) d.scene->d_shadow_nodes_quantised;
 		p.bvh_nodes_i = (const float4*) d.scene->d_shadow_nodes_interleaved;
-		if (p.bvh_width == 2 && !p.bvh_nodes_i) { printf("The scene holds no interleaved node pairs for the shadow rays (a scene object that was not made by this library?).\n"); return 1; }
-		for (int k = 0; k != 6; ++k) p.bvh_grid[k] = d.scene->shadow_grid[k];
+		if (!p.bvh_nodes_i) { printf("The scene holds no interleaved node pairs for the shadow rays (a scene object that was not made by this library?).\n"); return 1; }
 	}
 	if (any_textured_light) {
 		p.light_texture_texels = (const float4*) d.light_textures->d_texels; p.light_texture_dims = (const uint4*) d.light_textures->d_dims;
@@ -513,7 +510,6 @@ extern "C" int vkr_probe_rsqrt_exhaustive(const vkr_device_t* device, uint64_t* 
 
 extern "C" int vkr_trace_shadow_rays(const vkr_device_t* device, const vkr_scene_t* scene, uint32_t ray_count, const float* rays, uint8_t* out_occluded) {
 	if (!scene->d_shadow_nodes) { printf("Cannot trace shadow rays: the scene was loaded without acceleration structure.\n"); return 1; }
-	if (scene->shadow_bvh_width == 4) { printf("The shadow-ray probe walks node pairs; the scene was loaded with 4-wide nodes (VKR_BVH_WIDTH=4).\n"); return 1; }
 	VKR_CUDA_OK(cudaSetDevice(device->cuda_device), "Failed to select the CUDA device");
 	cudaStream_t stream = (cudaStream_t) device->stream;
 	float* d_rays = nullptr; uint8_t* d_out = nullptr;

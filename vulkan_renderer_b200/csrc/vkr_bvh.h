@@ -27,12 +27,10 @@ uint64_t lbvh_morton_code(const float centroid[3], const float lo[3], const floa
 // (void* like vkr_device_t::stream, so that this header needs no CUDA headers).
 int build_lbvh_device(const float* vertices, uint64_t triangle_count, void* stream, void** d_nodes, void** d_tris, void** d_tri_ids, uint64_t* node_count, uint32_t* max_depth);
 
-// Quantised node pairs for the trace warps of the shading kernels (vkr_trace.cuh: 32 bytes per pair, 16-bit box coordinates on a grid over the scene):
-// made on the device from the float pairs (vkr_lbvh_gpu.cu). grid = minimum xyz, cells per world unit xyz (shadow_grid_from_root below).
-int quantise_node_pairs_device(const void* d_nodes, uint64_t pair_count, const float grid[6], void** d_nodes_q, void* stream);
 // Interleaved node pairs (vkr_trace.cuh: the two children's numbers side by side, 64 bytes per pair), made on the device from the float pairs (vkr_lbvh_gpu.cu)
 int interleave_node_pairs_device(const void* d_nodes, uint64_t pair_count, void** d_nodes_i, void* stream);
-// The grid for a tree whose root pair (16 floats) is given: the scene's bounding box with two cells to spare on every side, 65536 cells per axis
+// The grid of the quantised node pairs (vkr_trace.cuh: quantise_node_pair) for a tree whose root pair (16 floats) is given: the scene's bounding box
+// with two cells to spare on every side, 65536 cells per axis; grid = minimum xyz, cells per world unit xyz
 void shadow_grid_from_root(const float* root_pair, float grid[6]);
 
 // 4-wide nodes collapsed from a BVH2 (vkr_bvh.cpp: build_bvh4_from_bvh2): groundwork for a traversal with half as many, fatter steps

@@ -87,7 +87,7 @@ extern "C" void vkr_destroy_scene(vkr_scene_t* scene, const vkr_device_t* device
 	free(scene->material_params);
 	void* dev_ptrs[] = { scene->d_quantized_positions, scene->d_normals_and_tex_coords, scene->d_material_indices, scene->d_material_params,
 		scene->d_shadow_nodes, scene->d_shadow_tris, scene->d_primary_nodes, scene->d_primary_tris, scene->d_primary_tri_ids,
-		scene->d_texture_data, scene->d_texture_dims, scene->d_texture_offsets, scene->d_shadow_nodes_quantised, scene->d_shadow_nodes_interleaved };
+		scene->d_texture_data, scene->d_texture_dims, scene->d_texture_offsets, scene->d_shadow_nodes_interleaved };
 	for (void* p : dev_ptrs) if (p) cudaFree(p);
 	memset(scene, 0, sizeof(*scene));
 }
@@ -142,32 +142,15 @@ static int scene_from_arrays(vkr_scene_t* scene, const vkr_device_t* device, con
 			if (which == bvh_builder_lbvh) build_lbvh(bvh, soup.data(), n);
 			if (which != bvh_builder_lbvh || bvh.max_depth >= 62) build_bvh(bvh, soup.data(), n);
 			scene->shadow_node_count = bvh.node_count; scene->shadow_max_depth = bvh.max_depth;
-			const char* width = getenv("VKR_BVH_WIDTH");
-			host_bvh4 wide;
-			if (width && !strcmp(width, "4") && bvh.max_depth < 62) { // experimental: 4-wide nodes for the kernel variant built with -DVKR_BVH_WIDTH=4 (up to 3 pushes per level)
-				build_bvh4_from_bvh2(wide, bvh);
-				if (3 * wide.max_depth + 2 <= 64) {
-					bvh.nodes = wide.nodes;
-					scene->shadow_node_count = wide.node_count; scene->shadow_max_depth = 3 * wide.max_depth; scene->shadow_bvh_width = 4;
-				}
-			}
 			if (bvh.max_depth >= 62 || upload(&scene->d_shadow_nodes, bvh.nodes.data(), bvh.nodes.size() * 4, device) || upload(&scene->d_shadow_tris, bvh.tris.data(), bvh.tris.size() * 4, device)) {
 				printf("Failed to construct an acceleration structure for the scene file at path %s.\n", file_path);
 				vkr_destroy_scene(scene, device); return 1;
 			}
 		}
-		if (scene->shadow_bvh_width == 2) { // the form the trace warps walk: 32-byte pairs with 16-bit boxes on a grid over the scene (vkr_trace.cuh)
-			float root[16];
-			if (cudaMemcpy(root, scene->d_shadow_nodes, sizeof(root), cudaMemcpyDeviceToHost) != cudaSuccess) { printf("Failed to read the root of the acceleration structure.\n"); vkr_destroy_scene(scene, device); return 1; }
-			shadow_grid_from_root(root, scene->shadow_grid);
-			if (quantise_node_pairs_device(scene->d_shadow_nodes, scene->shadow_node_count, scene->shadow_grid, &scene->d_shadow_nodes_quantised, device->stream)) {
-				printf("Failed to quantise the acceleration structure for the scene file at path %s.\n", file_path);
-				vkr_destroy_scene(scene, device); return 1;
-			}
-			if (interleave_node_pairs_device(scene->d_shadow_nodes, scene->shadow_node_count, &scene->d_shadow_nodes_interleaved, device->stream)) {
-				printf("Failed to interleave the acceleration structure for the scene file at path %s.\n", file_path);
-				vkr_destroy_scene(scene, device); return 1;
-			}
+		// the form the trace warps walk: the two children's numbers side by side (vkr_trace.cuh)
+		if (interleave_node_pairs_device(scene->d_shadow_nodes, scene->shadow_node_count, &scene->d_shadow_nodes_interleaved, device->stream)) {
+			printf("Failed to interleave the acceleration structure for the scene file at path %s.\n", file_path);
+			vkr_destroy_scene(scene, device); return 1;
 		}
 		// (b) primary rays: vertices as the shaders decode them (fma, mesh_quantization.glsl:38-45)
 		for (uint64_t i = 0; i != 3 * n; ++i) {

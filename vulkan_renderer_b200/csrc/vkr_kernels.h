@@ -37,12 +37,9 @@ struct shading_kernel_params {
 	const uint16_t* ltc0; const uint16_t* ltc1; int ltc_res, ltc_layers;
 	// acceleration structure
 	const float4* bvh_nodes; const float4* bvh_tris; uint32_t tri_count;
-	const uint4* bvh_nodes_q;        // the same node pairs quantised to 32 bytes (vkr_trace.cuh): what the trace warps walk
-	float bvh_grid[6];               // the grid of the quantised boxes: minimum xyz, cells per world unit xyz
-	const float4* bvh_nodes_i;       // the same node pairs with the two children interleaved (vkr_trace.cuh): what the trace warps of the VKR_INTERLEAVED_NODES edition walk
+	const float4* bvh_nodes_i;       // the same node pairs with the two children interleaved (vkr_trace.cuh): what the trace warps walk
 	int stack_depth;                 // traversal stack entries per lane (BVH depth + 2)
 	int polygon_sampling_technique;  // sample_polygon_technique_t (src/polygonal_light.h:30-66); 0..10 run vkr_related_work_kernel.cu
-	int bvh_width;                   // children per node of bvh_nodes: 2 (node pairs, default) or 4 (experimental, must equal the kernels' VKR_BVH_WIDTH)
 	int error_display;               // error_display_t (src/main.h:92-112); != 0 runs error_display_kernel (vkr_related_work_kernel.cu)
 	// light textures (vkr_light_textures_t); only the kernels of vkr_textured_light_kernel.cu read them. dims = {width, height, mip_count, -}, offsets in texels
 	const float4* light_texture_texels; const uint4* light_texture_dims; const unsigned long long* light_texture_offsets; uint32_t light_texture_count;
@@ -82,8 +79,6 @@ typedef cudaError_t vkr_related_work_probe_launcher_t(uint32_t technique, const 
 vkr_related_work_probe_launcher_t vkr_launch_related_work_probe_v3, vkr_launch_related_work_probe_v4, vkr_launch_related_work_probe_v5, vkr_launch_related_work_probe_v6, vkr_launch_related_work_probe_v7;
 // vkr_textured_related_work_kernel.cu: the related-work sampling techniques for frames with textured lights
 vkr_tile_launcher_t vkr_launch_textured_related_work_kernel_v3, vkr_launch_textured_related_work_kernel_v4, vkr_launch_textured_related_work_kernel_v5, vkr_launch_textured_related_work_kernel_v6, vkr_launch_textured_related_work_kernel_v7;
-// float node pairs -> quantised node pairs (vkr_lbvh_gpu.cu); d_nodes_q: 32 bytes per pair
-cudaError_t vkr_quantise_node_pairs(const float4* d_nodes, uint64_t pair_count, const float grid[6], uint4* d_nodes_q, cudaStream_t stream);
 // float node pairs -> interleaved node pairs (vkr_lbvh_gpu.cu); d_nodes_i: 64 bytes per pair
 cudaError_t vkr_interleave_node_pairs(const float4* d_nodes, uint64_t pair_count, float4* d_nodes_i, cudaStream_t stream);
 cudaError_t vkr_launch_visibility_kernel(const vkr::gbuffer_kernel_params& p, cudaStream_t stream);

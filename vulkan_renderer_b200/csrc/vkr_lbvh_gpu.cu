@@ -202,39 +202,6 @@ int build_lbvh_device(const float* vertices, uint64_t triangle_count, void* stre
 
 
 // ------------------------------------------------------------------------------------------------
-// Quantised node pairs for the trace warps (vkr_trace.cuh): one thread per pair
-namespace vkr {
-struct grid6 { float v[6]; };
-__global__ void quantise_pairs_kernel(const float4* __restrict__ nodes, unsigned long long count, grid6 grid, uint4* __restrict__ out) {
-	const unsigned long long i = (unsigned long long) blockIdx.x * blockDim.x + threadIdx.x;
-	if (i >= count) return;
-	unsigned w[8];
-	quantise_node_pair(nodes + 4 * i, grid.v, grid.v + 3, w);
-	out[2 * i] = make_uint4(w[0], w[1], w[2], w[3]);
-	out[2 * i + 1] = make_uint4(w[4], w[5], w[6], w[7]);
-}
-} // namespace vkr
-
-cudaError_t vkr_quantise_node_pairs(const float4* d_nodes, uint64_t pair_count, const float grid[6], uint4* d_nodes_q, cudaStream_t stream) {
-	if (!pair_count) return cudaSuccess;
-	vkr::grid6 g; for (int i = 0; i != 6; ++i) g.v[i] = grid[i];
-	vkr::quantise_pairs_kernel<<<(unsigned) ((pair_count + 255) / 256), 256, 0, stream>>>(d_nodes, (unsigned long long) pair_count, g, d_nodes_q);
-	return cudaGetLastError();
-}
-
-namespace vkr {
-// For the host code (vkr_host.cpp): allocates the quantised pairs and fills them from the float pairs on the device. grid: minimum xyz, cells per unit xyz.
-int quantise_node_pairs_device(const void* d_nodes, uint64_t pair_count, const float grid[6], void** d_nodes_q, void* stream) {
-	*d_nodes_q = nullptr;
-	if (cudaMalloc(d_nodes_q, 32 * (size_t) (pair_count ? pair_count : 1)) != cudaSuccess) { *d_nodes_q = nullptr; return 1; }
-	if (vkr_quantise_node_pairs((const float4*) d_nodes, pair_count, grid, (uint4*) *d_nodes_q, (cudaStream_t) stream) != cudaSuccess || cudaStreamSynchronize((cudaStream_t) stream) != cudaSuccess) {
-		cudaFree(*d_nodes_q); *d_nodes_q = nullptr; return 1;
-	}
-	return 0;
-}
-}
-
-// ------------------------------------------------------------------------------------------------
 // Interleaved node pairs for the trace warps (vkr_trace.cuh): one thread per pair
 namespace vkr {
 __global__ void interleave_pairs_kernel(const float4* __restrict__ nodes, unsigned long long count, float4* __restrict__ out) {

@@ -26,7 +26,6 @@ VKR_DEV void shade_light(bool on, const shading_point& sp, const ltc_state& l, c
 		if (vc == 0) on = false;
 		else prepare_psa<MAXP, BIASED>(pd, vc, v);
 	}
-	set_light_cone<TRACE, OPTIMAL>(q, lane, on, sp.position, light + L_FIXED + 16 * (MAXP - 1), (int) ldu(light, L_VERTEX_COUNT), p.bvh_nodes);
 	if (STRATEGY == VKR_STRATEGY_DIFFUSE_ONLY || STRATEGY == VKR_STRATEGY_DIFFUSE_GGX_MIS) {
 		if (on && pd.psa <= 0.0f) on = false;
 #pragma unroll 1
@@ -155,14 +154,8 @@ VKR_DEV void shade_light(bool on, const shading_point& sp, const ltc_state& l, c
 			// each sample right before its evaluation consumes the noise stream in the same order. One loop body serves
 			// both techniques and the end-of-light flush (s == S), so the kernel holds one copy of sample_psa and drain.
 			for (int s = 0; s <= S; ++s) {
-#if VKR_SHADING_LOCKSTEP == 1
-				if (TRACE && q.lockstep) shading_lockstep_barrier();
-#endif
 #pragma unroll 1
 				for (int j = 0; j != 2; ++j) {
-#if VKR_SHADING_LOCKSTEP == 2
-					if (TRACE && q.lockstep) shading_lockstep_barrier();
-#endif
 					bool has = on && s != S && (j == 0 || has_specular);
 					bool pre_vis = false; f3 w = zero, c = zero, c_occ = zero; float tmax = 0.0f;
 					if (has) {

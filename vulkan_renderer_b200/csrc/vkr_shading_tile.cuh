@@ -15,12 +15,7 @@ namespace vkr {
 constexpr int kTileW = 16, kTileH = 8, kShadeThreads = kTileW * kTileH;
 static_assert(kShadeThreads == 32 * kShadeWarps, "one shading warp per 8x4 patch");
 constexpr int kTraceThreads = 32 * kTraceWarps;
-#ifndef VKR_SHADE_REGS
-#define VKR_SHADE_REGS 128
-#endif
-#ifndef VKR_TRACE_REGS
-#define VKR_TRACE_REGS 56
-#endif
+constexpr int kShadeRegs = 128, kTraceRegs = 56;   // registers per thread of the shading and the trace warps after the split (setmaxnreg; DESIGN.md)
 // Dynamic shared memory of a tile: the constant block (constants_smem_bytes), then, with shadow rays, the ray streams of the shading warps (these
 // bytes) and the traversal stacks of the trace lanes (stack_depth ints each). tile_smem_bytes() (vkr_tile_launch.cuh) sizes launches by it.
 VKR_DEV constexpr size_t tile_streams_bytes(bool optimal) { return sizeof(float) * stream_floats_per_warp(optimal) * kShadeWarps; }
@@ -52,14 +47,13 @@ VKR_DEV void shade_tile(const shading_kernel_params& p, const LightShader& shade
 	if (TRACE) {
 		// --- role split: from here on the two kinds of warps never meet at a CTA-wide barrier again
 		if (warp >= kShadeWarps) {
-			asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" :: "n"(VKR_TRACE_REGS));
+			asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" :: "n"(kTraceRegs));
 			const int t = warp - kShadeWarps;
-			trace_stream<OPTIMAL>(smem_addr(stream_base + stream_floats_per_warp(OPTIMAL) * (t & (kShadeWarps - 1))), p.bvh_nodes, p.bvh_tris,
-				smem_addr(stack_base + p.stack_depth * 32 * t + lane), lane, p.stats, p.bvh_nodes_q,
-				make3(p.bvh_grid[0], p.bvh_grid[1], p.bvh_grid[2]), make3(p.bvh_grid[3], p.bvh_grid[4], p.bvh_grid[5]), p.bvh_nodes_i);
+			trace_stream<OPTIMAL>(smem_addr(stream_base + stream_floats_per_warp(OPTIMAL) * (t & (kShadeWarps - 1))), p.bvh_tris,
+				smem_addr(stack_base + p.stack_depth * 32 * t + lane), lane, p.stats, p.bvh_nodes_i);
 			return;
 		}
-		asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" :: "n"(VKR_SHADE_REGS));
+		asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" :: "n"(kShadeRegs));
 	}
 	if (threadIdx.x == 0) {
 		asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(mbar_addr), "r"(p.constants_bytes) : "memory");
@@ -118,28 +112,8 @@ VKR_DEV void shade_tile(const shading_kernel_params& p, const LightShader& shade
 #ifdef VKR_TRACE_STATS
 	q.stat_resolve_polls = 0; q.stat_candidates = 0;
 #endif
-	q.cone_set = false;
-	q.lockstep = false;
-#if VKR_SHADING_LOCKSTEP
-	if (TRACE) { // do all four shading warps of the tile have something to shade? (control word 3 of every stream is free for this)
-		const bool any_valid = __any_sync(kFullMask, valid) != 0;
-		if (lane == 0) sts_u32(q.base + 4u * (uint32_t) stream_control_at(OPTIMAL) + 12u, any_valid ? 1u : 0u);
-		shading_lockstep_barrier();
-		const uint32_t first_stream = smem_addr(stream_base);
-		bool all = true;
-		for (int w = 0; w != kShadeWarps; ++w) all = all && lds_u32(first_stream + 4u * (uint32_t) (stream_floats_per_warp(OPTIMAL) * w + stream_control_at(OPTIMAL)) + 12u) != 0u;
-		q.lockstep = all;
-	}
-#endif
-#if VKR_ANCHORED
-	if (TRACE) { // the origin path of this pixel (vkr_anchor.cuh): all of its shadow rays start from it
-		const uint32_t path = q.base + 4u * (uint32_t) stream_path_at(OPTIMAL) + 4u * (uint32_t) lane;
-		int tail = kTraversalDone, count = 0;
-		if (valid) count = find_origin_path(p.bvh_nodes, sp.position, &tail, [&](int k, uint32_t e) { sts_u32(path + 128u * (uint32_t) k, e); });
-		sts_u32(path + 128u * (uint32_t) kPathLevels, (uint32_t) tail);
-		sts_u32(path + 128u * (uint32_t) (kPathLevels + 1), (uint32_t) count);
-	}
-#endif
+	q.pad0 = false;
+	q.pad1 = false;
 	if (TRACE) {
 		float* origin = stream_base + stream_floats_per_warp(OPTIMAL) * warp + stream_origin_at(OPTIMAL);
 		origin[lane] = sp.position.x; origin[32 + lane] = sp.position.y; origin[64 + lane] = sp.position.z;

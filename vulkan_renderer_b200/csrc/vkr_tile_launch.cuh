@@ -2,7 +2,7 @@
 //
 // Included by the four kernel translation units (vkr_shading_kernel.cu, vkr_textured_light_kernel.cu, vkr_related_work_kernel.cu,
 // vkr_textured_related_work_kernel.cu); each of them is compiled once per bound of the light vertex count and exports one entry point per bound.
-// Everything here has internal linkage: VKR_BVH_WIDTH and the stream layout are compile-time choices of each unit that variant builds override.
+// Everything here has internal linkage: every unit is compiled with its own VKR_MAXV_TU.
 #pragma once
 #include "vkr_shading_tile.cuh"
 
@@ -16,7 +16,7 @@
 #define VKR_TILE_LAUNCHER(prefix) VKR_CONCAT(prefix, VKR_MAXV_TU)
 
 #ifndef VKR_TRACED_CTAS_PER_SM
-#define VKR_TRACED_CTAS_PER_SM 2   // CTAs per SM the register allocation of the kernels with shadow rays is made for (tuning knob, with VKR_SHADE_REGS / VKR_TRACE_REGS)
+#define VKR_TRACED_CTAS_PER_SM 2   // CTAs per SM the register allocation of the kernels with shadow rays is made for (with kShadeRegs / kTraceRegs, vkr_shading_tile.cuh)
 #endif
 // __launch_bounds__ of every tile kernel: the shading warps, plus the trace warps when it traces shadow rays
 #define VKR_TILE_LAUNCH_BOUNDS(TRACE) __launch_bounds__((TRACE) ? kShadeThreads + kTraceThreads : kShadeThreads, (TRACE) ? VKR_TRACED_CTAS_PER_SM : 3)
@@ -28,7 +28,6 @@ static bool traces_shadow_rays(const shading_kernel_params& p) { return p.trace_
 // What every tile kernel that shades radiance needs; light_textures: the kernel reads the light textures.
 static bool tile_launch_valid(const shading_kernel_params& p, bool light_textures) {
 	if (p.stack_depth < 2 || p.stack_depth > kMaxStackDepth) return false;
-	if (traces_shadow_rays(p) && p.bvh_width != VKR_BVH_WIDTH) return false; // the scene's BVH layout must be the one these kernels walk
 	return !light_textures || (p.light_texture_texels && p.light_texture_dims && p.light_texture_offsets && p.light_texture_count != 0);
 }
 

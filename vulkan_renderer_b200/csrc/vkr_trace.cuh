@@ -85,9 +85,9 @@ VKR_DEV float slab_reciprocal(float x) {
 	return (fabsf(x) < 5.421010862427522e-20f) ? copysignf(__int_as_float(0x7f800000), x) : y;   // 2^-64
 }
 
-// Ray in the form the slab test wants: id = 1/d, oid = o/d. GUARDED = false is for the compile-time editions of the trace warps' loop
-// (vkr_ray_stream.cuh): their rays point from a surface point to a point on a light, normalised, so a nonzero component is far above 2^-64 for any
-// scene with coordinates above 1e-12.
+// Ray in the form the slab test wants: id = 1/d, oid = o/d. GUARDED = false leaves out the guard, which is sound for the shading kernels' shadow rays
+// (vkr_ray_stream.cuh): they point from a surface point to a point on a light, normalised, so a nonzero component is far above 2^-64 for any scene
+// with coordinates above 1e-12.
 struct ray_slabs { f3 id, oid; };
 template <bool GUARDED = true>
 VKR_DEV ray_slabs make_slabs(f3 o, f3 d) {
@@ -219,7 +219,7 @@ VKR_DEV bool occluded_interleaved(const float* __restrict__ pairs16, const float
 }
 
 // ---------------------------------------------------------------------------------------------------------------------------------------
-// Quantised node pairs: an edition of the trace warps' loop with half the bytes per visit (VKR_QUANTISED_NODES, vkr_ray_stream.cuh). A pair shrinks from
+// Quantised node pairs: a node layout with half the bytes per visit, tried for the trace warps and not taken (DESIGN.md section 3). A pair shrinks from
 // 64 to 32 bytes -- one sector per lane -- by storing the two child boxes as 16-bit coordinates on a grid over the scene's bounding box:
 //   word 0..2  child 0: x, y, z as (low | high << 16)      word 3..5  child 1      word 6, 7  the two child references (as in the float pairs)
 // Boxes are rounded outwards to the grid and one more cell (below), so the test stays conservative; the triangle predicate is untouched and hit / miss
@@ -253,7 +253,7 @@ VKR_DEV bool ray_box_grid(unsigned wx, unsigned wy, unsigned wz, const ray_grid&
 	*t_near = tn;
 	return tn <= tf;
 }
-// One float node pair -> its quantised form (8 words). Used by the quantisation kernel (vkr_lbvh_gpu.cu) and by the CPU tests.
+// One float node pair -> its quantised form (8 words), for the CPU tests.
 VKR_DEV void quantise_node_pair(const float4* __restrict__ pair, const float* grid_min, const float* grid_scale, unsigned* out8) {
 	const float4 q0 = pair[0], q1 = pair[1], q2 = pair[2], q3 = pair[3];
 	const float c[2][3] = { { q0.x, q0.y, q0.z }, { q1.z, q1.w, q2.x } }, h[2][3] = { { q0.w, q1.x, q1.y }, { q2.y, q2.z, q2.w } };
@@ -267,7 +267,7 @@ VKR_DEV void quantise_node_pair(const float4* __restrict__ pair, const float* gr
 		}
 	out8[6] = __float_as_uint(q3.x); out8[7] = __float_as_uint(q3.y);
 }
-// Per-thread any-hit query over quantised pairs: the reference form of the trace warps' loop (vkr_ray_stream.cuh), run on the CPU against occluded().
+// Per-thread any-hit query over quantised pairs, run on the CPU against occluded().
 VKR_DEV bool occluded_grid(const unsigned* __restrict__ pairs8, const float4* __restrict__ tris, const float* grid_min, const float* grid_scale, f3 o, f3 d, float tmin, float tmax, int* stack, int stride, int* visits) {
 	if (!(tmax > tmin)) return false;
 	const ray_grid g = make_ray_grid(o, d, make3(grid_min[0], grid_min[1], grid_min[2]), make3(grid_scale[0], grid_scale[1], grid_scale[2]));
@@ -331,8 +331,7 @@ VKR_DEV bool occluded(const bvh_view& bvh, f3 o, f3 d, float tmin, float tmax, i
 
 // One step through a 4-wide node (vkr_bvh.h: host_bvh4; 8 x float4 per node: child c has centre and half extent at floats [6c, 6c + 6), the four
 // references as int bits in the seventh float4). Tests the four boxes, returns the reference of the nearest hit child and hands the other hit
-// children (inner nodes and leaves alike) to push(); returns kTraversalDone if no child is hit. Shared by occluded4() below (tested on the CPU)
-// and by the experimental 4-wide form of the trace warps' loop (vkr_ray_stream.cuh, VKR_BVH_WIDTH == 4).
+// children (inner nodes and leaves alike) to push(); returns kTraversalDone if no child is hit. The step of occluded4() below (tested on the CPU).
 template <class Push>
 VKR_DEV int bvh4_descend_step(const float4* __restrict__ nodes4, int node, const ray_slabs& r, float tmin, float tmax, Push&& push) {
 	const float4* nd = nodes4 + 8 * (size_t) node;
